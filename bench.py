@@ -8,7 +8,11 @@ One "step" = one full pass of the hot path over one batch: 250 denoising steps f
 Independent prompts shard across GPUs with no data-path collective (weak scaling); the finished
 latents are all-gathered once per step (tiny).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
+
+`--dump-outputs DIR` writes what the timed path computed in its last timed step (the sampled latents
+this rank returns, float32) as DIR/latents.npy; the inputs are drawn from fixed seeds, so two builds run
+with the same arguments can be compared output for output.
 
 `--impl reference` times the reference algorithm's CPU path (the oracle port -- /root/reference
 is a Python tree that cannot travel to the GPU box) on a bounded sample of the same workload.
@@ -44,6 +48,8 @@ def parse():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--denoise-steps", type=int, default=DENOISE_STEPS, help=argparse.SUPPRESS)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs as DIR/<name>.npy (float32)")
     return ap.parse_args()
 
 
@@ -203,7 +209,7 @@ class ClockSampler:
 def gpu_reference_leg(torch, dev, state_dict, B, nsteps, randn_d, ctx_d):
     """The reference's GPU arithmetic (stock eager PyTorch under bf16 autocast: cuBLAS + SDPA-flash, the
     reference's per-step recomputation and sampler launches left in; baseline/torch_eager.py) on the same
-    B200, same workload, timed BEFORE the repo's arm in the same process (SURVEY.md 8d timing protocol).
+    GPU, same workload, timed BEFORE the repo's arm in the same process (SURVEY.md 8d timing protocol).
     Bounded sample: `sample_steps` of the 250 denoising steps for the full 8-prompt batch, 3 repeats after a
     warm-up, extrapolated linearly in steps (every step launches the same kernels on the same shapes)."""
     from baseline.torch_eager import EagerDiT, euler_edm_cfg_steps
@@ -275,11 +281,14 @@ def run_ours(args):
     tables = pipeline.edm_cfg_tables(nsteps, CFG_SCALE, B, dev)
     gathered = torch.empty(n_gpus * B, 12, 32, 32, device=dev) if world > 1 else None
 
+    last = {}
+
     def one_step_device():
         lat = pipeline.sample_t23d(model, randn_d, {"crossattn": ctx_d}, {"crossattn": uc_d}, nsteps,
                                    CFG_SCALE, tables)
         if world > 1:
             dist.all_gather_into_tensor(gathered, lat)
+        last["latents"] = lat
         return lat
 
     def one_step_e2e():
@@ -321,6 +330,11 @@ def run_ours(args):
     clk = clocks.stop() if rank == 0 else None
     ms_step = ms_total / args.steps
     value = B * n_gpus / (ms_step / 1e3)
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, t in last.items():
+            np.save(os.path.join(args.dump_outputs, f"{name}.npy"), t.detach().float().cpu().numpy())
 
     ms_e2e_total, _ = timed(one_step_e2e, args.steps, 1)
     e2e_value = B * n_gpus / (ms_e2e_total / args.steps / 1e3)
@@ -374,7 +388,7 @@ def run_ours(args):
 
     line = None
     if rank == 0:
-        # ---- roofline of the dominant kernel (tcgen05 GEMM): instrumented pass over one forward,
+        # ---- roofline of the dominant kernel (wgmma GEMM): instrumented pass over one forward,
         # CUDA events around every GEMM launch on the launching stream.
         peaks = {}
         try:
@@ -385,7 +399,7 @@ def run_ours(args):
         peak_tf = peaks.get("bf16_tflops_sustained")
         peak_src = "MEASURED_PEAKS.json bf16_tflops_sustained (kernel timed inside a long step)"
         if not peak_tf:
-            peak_tf, peak_src = 1400.0, "fallback (B200_PROFILING.md sustained ~1.4 PFLOP/s)"
+            peak_tf, peak_src = 989.0, "H100 SXM data sheet, dense BF16 at 700 W (not a measured rate)"
         ev, flops = [], []
         real_gemm = ops.gemm
 
@@ -415,19 +429,13 @@ def run_ours(args):
         gemm_fl = sum(f for f, _ in big)
         achieved = gemm_fl / (gemm_ms / 1e3) / 1e12 if gemm_ms > 0 else 0.0
         traffic, traffic_src = None, None
-        try:   # dram bytes of the dominant launch from this round's `ncu --set full` capture (tools/summarize_ncu.py)
-            with open(os.path.join(ROOT, "profiles", "r2_gemm_traffic.json")) as f:
-                tj = json.load(f)
-            traffic, traffic_src = tj["dram_bytes_per_launch"], tj["source"]
-        except Exception:
-            pass
-        roofline = {"kernel": "ln3::gemm2_bf16_kernel (tcgen05 cta_group::2, 256x256x64 per CTA pair, fused epilogues)",
+        roofline = {"kernel": "ln3::gemm_bf16_kernel (wgmma, 128x128x64 tiles, TMA ring, fused epilogues)",
                     "bound": "tensor", "achieved": achieved, "peak": peak_tf, "unit": "TFLOP/s",
                     "frac": achieved / peak_tf, "peak_source": peak_src,
                     "traffic": traffic, "traffic_source": traffic_src,
                     "launches_measured": len(big), "avg_launch_us": 1e3 * gemm_ms / max(len(big), 1),
                     "flops_per_launch_avg": gemm_fl / max(len(big), 1),
-                    "note": "events add launch gaps; gemm share of the forward in profiles/"}
+                    "note": "events add launch gaps"}
         model_tf = FLOPS_EXECUTED_PER_FORWARD_PER_SAMPLE * 2 * B * nsteps / (ms_step / 1e3) / 1e12
         model_tf_ref = FLOPS_PER_FORWARD_PER_SAMPLE * 2 * B * nsteps / (ms_step / 1e3) / 1e12
 
@@ -610,7 +618,7 @@ def run_ours(args):
             del ce, de
             cond = {"clip_text_prompts_per_s": 8 / t_ms * 1e3, "i23d_images_per_s": 8 / i_ms * 1e3,
                     "ms_per_8_prompts": t_ms, "ms_per_8_images_clip_plus_dino": i_ms,
-                    "what": "frozen conditioner towers on the tcgen05 GEMM / FMHA kernels, 8 prompts or images per call"}
+                    "what": "frozen conditioner towers on the wgmma GEMM / FMHA kernels, 8 prompts or images per call"}
         except Exception as e:  # noqa
             cond = {"error": repr(e)}
 

@@ -1,11 +1,11 @@
-/* libln3b200 -- C ABI of the B200-native LN3Diff generation hot path.
+/* libln3b200 -- C ABI of the H100-native (sm_90a) LN3Diff generation hot path.
  *
  * Drop-in boundary (SURVEY.md section 8b): every entry point takes a plain-C argument struct
  * of raw device pointers, explicit sizes/strides and enums, plus the CUDA stream as `void*`
  * (a cudaStream_t).  No torch types, no allocation, no retained pointers, no host
  * synchronisation: callers own every buffer (including workspaces).  All entry points return
  * LN3_OK (0) or a negative LN3_E* code; ln3_last_error() returns the thread-local message.
- * There is deliberately no CPU fallback: on a box without an sm_100 GPU every compute call
+ * There is deliberately no CPU fallback: on a box without an sm_90 GPU every compute call
  * fails with LN3_ECUDA.
  *
  * Each entry point cites the reference code (NIRVANALAN/LN3Diff, paths relative to the
@@ -38,11 +38,11 @@ unsigned long long ln3_launch_count(void);
  * the library: callers add the graph's kernel-node count per replay to keep the tally honest. */
 void ln3_add_launch_count(unsigned long long n);
 
-/* ------------------------------------------------------------------ GEMM (tcgen05 + TMA)
+/* ------------------------------------------------------------------ GEMM (wgmma + TMA)
  * out = epilogue(A[M,K] . W[N,K]^T): replaces every nn.Linear on the path
  *   dit/dit_models_xformers.py:231-323 (adaLN_modulation, FusedMLP), vit/vision_transformer.py:
  *   106-124 (qkv, proj), ldm/modules/attention.py:245-307 (to_q/k/v/out), dit/dit_decoder.py.
- * A, W bf16 row-major (K contiguous); fp32 accumulation in TMEM.
+ * A, W bf16 row-major (K contiguous); fp32 accumulation in registers.
  * Epilogue: + bias[N] (fp32, optional) -> activation -> one of
  *   LN3_OUT_BF16       out bf16 [M, ldo]
  *   LN3_OUT_F32        out f32  [M, ldo]
@@ -77,10 +77,7 @@ typedef struct ln3_gemm_args {
   int head_norm_nsec;
   int head_norm_sec_cols;
   float head_norm_eps;
-  /* optional scratch for the stream-K tail of the CTA-pair kernel: ln3_gemm_workspace_bytes() bytes of
-   * device memory, 256-byte aligned, ZEROED ONCE by the caller (the kernel leaves it zeroed), never shared
-   * by GEMMs that may run concurrently.  With T output tiles on P CTA pairs the last T % P tiles are split
-   * along K over all pairs instead of leaving P - T % P pairs idle for a whole tile.  NULL -> plain tiles. */
+  /* reserved scratch (the kernel needs none: ln3_gemm_workspace_bytes() returns 0); ignored. */
   void* workspace;
   size_t workspace_bytes;
 } ln3_gemm_args;
@@ -89,7 +86,7 @@ size_t ln3_gemm_workspace_bytes(void);
 
 int ln3_gemm_bf16(const ln3_gemm_args* args, void* stream);
 
-/* ------------------------------------------------------------------ attention (tcgen05)
+/* ------------------------------------------------------------------ attention (wgmma)
  * out[b, i, h*64:(h+1)*64] = softmax(q_h k_h^T * scale) v_h, no mask: replaces
  * xformers.ops.memory_efficient_attention at vit/vision_transformer.py:114-118 (packed qkv of
  * MemEffAttention), ldm/modules/attention.py:279-307 (cross-attention, incl. its three
@@ -107,8 +104,7 @@ typedef struct ln3_fmha_args {
   int B, H, Lq, Lkv, head_dim;
   long long q_ld, q_bs, k_ld, k_bs, v_ld, v_bs, o_ld, o_bs; /* elements */
   float scale;
-  /* optional second K/V source appended after the first along the sequence (Lkv must then be a
-   * multiple of 128 for the two-warpgroup kernel; the default kernel takes any Lkv): the step-invariant DINO tokens the I23D blocks concatenate to the latent
+  /* optional second K/V source appended after the first along the sequence (any Lkv / Lkv2): the step-invariant DINO tokens the I23D blocks concatenate to the latent
    * tokens for self-attention (dit/dit_models_xformers.py:522-530) -- their K/V are cached per
    * prompt and never copied.  k2/v2 NULL -> unused. */
   const void* k2;

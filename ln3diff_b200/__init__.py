@@ -1,4 +1,4 @@
-"""ln3diff_b200 -- B200-native (sm_100a) implementation of the LN3Diff generation hot path.
+"""ln3diff_b200 -- H100-native (sm_90a) implementation of the LN3Diff generation hot path.
 
 Host side mirrors the reference's Python interface for the path (DiT_models, samplers, Triplane /
 ImportanceRenderer); the device work is hand-written CUDA in libln3b200.so behind a C ABI

@@ -1,7 +1,6 @@
-// Shared device helpers for the sm_100a kernels of libln3b200: mbarrier, TMA
-// (cp.async.bulk.tensor), tcgen05 (UMMA / TMEM) inline-PTX wrappers and the shared-memory /
-// instruction descriptor encoders.  Bit layouts follow the PTX ISA "tcgen05" chapter (the
-// same fields CUTLASS names UMMA::SmemDescriptor / UMMA::InstrDescriptor).
+// Shared device helpers for the sm_90a kernels of libln3b200: mbarrier, TMA (cp.async.bulk.tensor),
+// wgmma inline-PTX wrappers and the shared-memory matrix descriptor encoder.  Bit layouts follow the
+// PTX ISA "asynchronous warpgroup level matrix" section (the fields CUTLASS names GmmaDescriptor).
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -140,92 +139,56 @@ __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk
 __device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 __device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
-// ------------------------------------------------------------------ tcgen05 / TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// tcgen05.commit: arrive on `bar` once all previously issued tcgen05.mma of this thread finish.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   smem_u32(bar))
-               : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem], kind::f16 (bf16/fp16 inputs, fp32 accumulate).
-__device__ __forceinline__ void umma_f16_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                            uint32_t idesc, uint32_t accumulate) {
+// ------------------------------------------------------------------ wgmma (warpgroup MMA)
+// Every wgmma of a warpgroup is preceded by wgmma_fence() (orders the accumulator / A registers written by
+// ordinary instructions), issued, committed as one group and waited for before its registers are read.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// Keeps the compiler from moving accesses of an accumulator across the asynchronous MMA that owns it.
+__device__ __forceinline__ void reg_fence(float& r) { asm volatile("" : "+f"(r)::"memory"); }
+// D[64 x 128] (fp32, registers) (+)= A[smem desc] * B[smem desc]^T, both K-major bf16.  scale_d = 0: D = A * B.
+__device__ __forceinline__ void wgmma_m64n128k16_ss(float* d, uint64_t desc_a, uint64_t desc_b, uint32_t scale_d) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(desc_a), "l"(desc_b), "r"(scale_d));
 }
-// A operand from tensor memory (lane = row, 32-bit column c = K elements 2c, 2c+1), B from shared memory.
-__device__ __forceinline__ void umma_f16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc,
-                                            uint32_t accumulate) {
+// D[64 x 64] (fp32) (+)= A[registers: m16n8k16-style A fragments, 16 rows per warp] * B[smem desc], B MN-major
+// (a row-major K x N tile, N contiguous, transposed by the instruction).  scale_d = 0: D = A * B.
+__device__ __forceinline__ void wgmma_m64n64k16_rs_tb(float* d, const uint32_t* a, uint64_t desc_b, uint32_t scale_d) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "setp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, 1;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(scale_d));
 }
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+
+// Shared-memory matrix descriptor (64 bit):
+//   [0,14)  start address >> 4        [16,30) leading-dim byte offset >> 4
+//   [32,46) stride-dim byte offset>>4 [49,52) base offset     [62,64) layout: 1 = 128B swizzle
+// K-major, SWIZZLE_128B tile whose rows are 128 bytes (64 bf16): 8-row groups are `sbo` bytes apart (1024 for
+// a dense tile); LBO is unused for swizzled K-major operands.  A K step of 16 elements inside the 128-byte row
+// advances the start address by 32 bytes (+2 in the descriptor).
+// MN-major, SWIZZLE_128B: 64 MN-elements (128 B) contiguous, k-rows 128 B apart, 8-k-row groups `sbo` bytes
+// apart, further 64-element MN groups `lbo` bytes apart.  A K step of 16 rows advances 2048 bytes (+128).
+// Tiles start on a 1024-byte boundary (the swizzle pattern repeats every 8 rows of 128 bytes).
+__device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes,
+                                                         uint32_t sbo_bytes) {
+  uint64_t d = 0;
+  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
+  d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
+  d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
+  d |= static_cast<uint64_t>(1) << 62;
+  return d;
 }
-// 32 lanes x 32 columns of 32-bit: thread t of the warp receives lane (warp%4)*32+t, cols c..c+31.
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t* v) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]),
-        "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]),
-        "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]),
-        "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]),
-        "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() {
-  asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_st_32x32(uint32_t taddr, const uint32_t* v) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-      "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]),
-      "r"(v[8]), "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]),
-      "r"(v[16]), "r"(v[17]), "r"(v[18]), "r"(v[19]), "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]),
-      "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]), "r"(v[28]), "r"(v[29]), "r"(v[30]), "r"(v[31])
-      : "memory");
-}
-// one 32-bit TMEM column (lane = thread's row): scratch exchange between warps that share TMEM lanes
-__device__ __forceinline__ void tmem_st_32x1(uint32_t taddr, uint32_t v) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x1.b32 [%0], {%1};" ::"r"(taddr), "r"(v) : "memory");
-}
-__device__ __forceinline__ uint32_t tmem_ld_32x1(uint32_t taddr) {
-  uint32_t v;
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x1.b32 {%0}, [%1];" : "=r"(v) : "r"(taddr) : "memory");
-  return v;
-}
+
 // Programmatic dependent launch: the kernel may start while its stream predecessor is still running;
 // pdl_wait() returns once every prerequisite grid has completed and its memory is visible (a no-op for a
 // normal launch), pdl_launch_dependents() lets the NEXT kernel's CTAs be scheduled as ours retire.
@@ -238,9 +201,7 @@ __device__ __forceinline__ int ld_acquire_gpu(const int* p) {
   return v;
 }
 
-// One lane of the (converged) warp.  Code that feeds tcgen05.mma should run warp-uniformly and guard
-// only the issue itself with this: inside an `if (lane == 0)` region ptxas cannot prove descriptors
-// uniform and wraps every UTCHMMA in an ELECT / R2UR.BROADCAST waterfall (~100 cycles per MMA).
+// One elected lane of the (converged) warp.
 __device__ __forceinline__ bool elect_one_sync() {
   uint32_t pred;
   asm volatile(
@@ -256,7 +217,8 @@ __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
 __device__ __forceinline__ void named_bar_arrive(int id, int nthreads) {
   asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
-// Packed fp32x2 arithmetic (sm_100: FFMA2 / FADD2 -- one issue slot for two lanes of work).
+// fp32 pairs held in one 64-bit value; fma2 evaluates both lanes with scalar FMAs (same rounding as the
+// packed form: one fma.rn per lane).
 __device__ __forceinline__ uint64_t pk2(float lo, float hi) {
   uint64_t d;
   asm("mov.b64 %0, {%1, %2};" : "=l"(d) : "f"(lo), "f"(hi));
@@ -265,159 +227,51 @@ __device__ __forceinline__ uint64_t pk2(float lo, float hi) {
 __device__ __forceinline__ void upk2(uint64_t v, float& lo, float& hi) {
   asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
 }
-__device__ __forceinline__ uint64_t fma2(uint64_t a, uint64_t b, uint64_t c) {
-  uint64_t d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
-}
-__device__ __forceinline__ uint64_t add2(uint64_t a, uint64_t b) {
-  uint64_t d;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-__device__ __forceinline__ float fmax3(float a, float b, float c) {
-  float d;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(d) : "f"(a), "f"(b), "f"(c));
-  return d;
-}
 __device__ __forceinline__ float fast_exp2(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, uint32_t* v) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]),
-        "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]),
-        "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
+__device__ __forceinline__ uint64_t fma2(uint64_t a, uint64_t b, uint64_t c) {
+  float a0, a1, b0, b1, c0, c1;
+  upk2(a, a0, a1);
+  upk2(b, b0, b1);
+  upk2(c, c0, c1);
+  return pk2(fmaf(a0, b0, c0), fmaf(a1, b1, c1));
 }
 
-// ------------------------------------------------------------------ CTA pairs (cta_group::2)
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// shared::cluster address of `smem_ptr`'s location in CTA `rank` of the cluster
-__device__ __forceinline__ uint32_t mapa_u32(const void* smem_ptr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_u32(smem_ptr)), "r"(rank));
-  return r;
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// Same without the release fence.  .release.cluster compiles to MEMBAR.ALL.GPU + ERRBAR, i.e. it waits for
-// every global store the warp has in flight (an epilogue's whole output) -- 9 % of the GEMM's stall
-// samples.  Use it where only tcgen05 traffic must be ordered (tcgen05.fence::before_thread_sync does that).
-__device__ __forceinline__ void mbar_arrive_cluster_relaxed(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.relaxed.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// TMA load of one CTA of a pair; completion bytes are credited to the barrier at `mbar_cluster_addr`
-// (the leader CTA's full barrier).
-__device__ __forceinline__ void tma_load_2d_2sm(void* smem_dst, const CUtensorMap* m, uint32_t mbar_cluster_addr,
-                                                int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4}], [%2];" ::"r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(mbar_cluster_addr), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_2sm() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem of both CTAs] (+)= A[smem, 128 rows per CTA] * B[smem, N/2 rows per CTA]; issued by the leader.
-__device__ __forceinline__ void umma_f16_ss_2sm(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                                uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive (once the leader's previously issued MMAs retire) on the barrier at the same offset in every
-// CTA of `cta_mask`
-__device__ __forceinline__ void umma_commit_2sm(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"(cta_mask)
-      : "memory");
-}
-
-// ------------------------------------------------------------------ descriptors
-// Shared-memory matrix descriptor (64 bit):
-//   [0,14)  start address >> 4        [16,30) leading-dim byte offset >> 4
-//   [32,46) stride-dim byte offset>>4 [46,48) version (1 on sm_100)
-//   [49,52) base offset               [61,64) layout: 0 none, 2 = 128B swizzle, 4 = 64B, 6 = 32B
-// K-major, SWIZZLE_128B tile whose rows are 128 bytes (64 bf16): 8-row groups are `sbo` bytes
-// apart (1024 for a dense tile); LBO is ignored by the hardware for swizzled K-major operands.
-// MN-major, SWIZZLE_128B: 64 MN-elements (128 B) contiguous, k-rows 128 B apart, 8-k-row groups
-// `sbo` bytes apart, further 64-element MN groups `lbo` bytes apart.
-__device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes,
-                                                         uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-  d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
-  return d;
-}
-// Instruction descriptor for kind::f16 with bf16 A/B and fp32 D.
-//   [4,6) D fmt (1 = f32)  [7,10) A fmt (1 = bf16)  [10,13) B fmt  [15] A major (0 = K)
-//   [16] B major           [17,23) N >> 3           [24,29) M >> 4
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int m, int n, int a_mn_major,
-                                                       int b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (static_cast<uint32_t>(a_mn_major) << 15) |
-         (static_cast<uint32_t>(b_mn_major) << 16) | (static_cast<uint32_t>(n >> 3) << 17) |
-         (static_cast<uint32_t>(m >> 4) << 24);
-}
-
-// ------------------------------------------------------------------ 256-bit global accesses
-// One lane moves a full 32-byte sector per instruction (LDG/STG.E.ENL2.256 on sm_100): half the L1
-// wavefronts of the 128-bit forms for the thread-per-row epilogues.  32-byte aligned addresses.
+// ------------------------------------------------------------------ 32-byte global accesses
+// Eight consecutive fp32 / 32-bit words as two 128-bit accesses (32-byte aligned addresses).
 __device__ __forceinline__ void ldg256_na(const void* p, float* v) {
-  asm volatile("ld.global.L1::no_allocate.v8.f32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=f"(v[0]), "=f"(v[1]), "=f"(v[2]), "=f"(v[3]), "=f"(v[4]), "=f"(v[5]), "=f"(v[6]), "=f"(v[7])
-               : "l"(p));
+  asm volatile("ld.global.L1::no_allocate.v4.f32 {%0,%1,%2,%3}, [%4];"
+               : "=f"(v[0]), "=f"(v[1]), "=f"(v[2]), "=f"(v[3]) : "l"(p));
+  asm volatile("ld.global.L1::no_allocate.v4.f32 {%0,%1,%2,%3}, [%4+16];"
+               : "=f"(v[4]), "=f"(v[5]), "=f"(v[6]), "=f"(v[7]) : "l"(p));
 }
-// L2 evict_last forms: the fp32 residual stream (50 MB at DiT-L/2 B'=16) is read and re-written by three passes per
-// block with 25-100 MB GEMM streams in between; marking its lines evict_last keeps them in the 126 MB L2.
+// L2 evict_last forms: the fp32 residual stream is read and re-written by three passes per block with GEMM
+// operand streams in between; marking its lines evict_last keeps them in L2.
 __device__ __forceinline__ void ldg256_na_el(const void* p, float* v) {
-  asm volatile("ld.global.L1::no_allocate.L2::evict_last.v8.f32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=f"(v[0]), "=f"(v[1]), "=f"(v[2]), "=f"(v[3]), "=f"(v[4]), "=f"(v[5]), "=f"(v[6]), "=f"(v[7])
-               : "l"(p));
+  asm volatile(
+      "{\n\t.reg .b64 pol;\n\t"
+      "createpolicy.fractional.L2::evict_last.b64 pol, 1.0;\n\t"
+      "ld.global.L1::no_allocate.L2::cache_hint.v4.f32 {%0,%1,%2,%3}, [%8], pol;\n\t"
+      "ld.global.L1::no_allocate.L2::cache_hint.v4.f32 {%4,%5,%6,%7}, [%8+16], pol;\n\t}\n"
+      : "=f"(v[0]), "=f"(v[1]), "=f"(v[2]), "=f"(v[3]), "=f"(v[4]), "=f"(v[5]), "=f"(v[6]), "=f"(v[7])
+      : "l"(p));
 }
 __device__ __forceinline__ void stg256_f32_el(void* p, const float* v) {
-  asm volatile("st.global.L2::evict_last.v8.f32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "f"(v[0]), "f"(v[1]), "f"(v[2]),
-               "f"(v[3]), "f"(v[4]), "f"(v[5]), "f"(v[6]), "f"(v[7])
-               : "memory");
+  asm volatile(
+      "{\n\t.reg .b64 pol;\n\t"
+      "createpolicy.fractional.L2::evict_last.b64 pol, 1.0;\n\t"
+      "st.global.L2::cache_hint.v4.f32 [%0], {%1,%2,%3,%4}, pol;\n\t"
+      "st.global.L2::cache_hint.v4.f32 [%0+16], {%5,%6,%7,%8}, pol;\n\t}\n" ::"l"(p),
+      "f"(v[0]), "f"(v[1]), "f"(v[2]), "f"(v[3]), "f"(v[4]), "f"(v[5]), "f"(v[6]), "f"(v[7])
+      : "memory");
 }
 __device__ __forceinline__ void stg256_f32(void* p, const float* v) {
-  asm volatile("st.global.v8.f32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "f"(v[0]), "f"(v[1]), "f"(v[2]),
-               "f"(v[3]), "f"(v[4]), "f"(v[5]), "f"(v[6]), "f"(v[7])
+  asm volatile("st.global.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(p), "f"(v[0]), "f"(v[1]), "f"(v[2]), "f"(v[3])
                : "memory");
-}
-__device__ __forceinline__ void stg256_b32(void* p, const uint32_t* v) {
-  asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "r"(v[0]), "r"(v[1]), "r"(v[2]),
-               "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7])
+  asm volatile("st.global.v4.f32 [%0+16], {%1,%2,%3,%4};" ::"l"(p), "f"(v[4]), "f"(v[5]), "f"(v[6]), "f"(v[7])
                : "memory");
 }
 
@@ -454,12 +308,10 @@ __device__ __forceinline__ float gelu_erf_fast(float x) {
   const float w = (q * t) * (e * x);                            // x * 0.5 erfc(z), sign of x
   return fmaxf(x, 0.f) - fabsf(w);
 }
-// erf-GELU for the fc1 epilogue of the CTA-pair GEMM, two elements at a time on the packed fp32x2 FMA pipe and
-// WITHOUT the XU:  GELU(x) = x * Phi(x),  Phi(x) = sat(0.5 + x * Q(min(x^2, 16))),  Q an even polynomial of degree
+// erf-GELU for the fc1 epilogue of the GEMM, two elements at a time on the FMA pipe and WITHOUT the MUFU:
+// GELU(x) = x * Phi(x),  Phi(x) = sat(0.5 + x * Q(min(x^2, 16))),  Q an even polynomial of degree
 // 8 in u = x^2 fitted (x^2-weighted Chebyshev least squares on |x| <= 4) to (Phi(x) - 0.5) / x.  fma.sat clamps
-// Phi to [0, 1], which is also the right limit for |x| > 4 (x Q(16) = +-0.49997 |x| / 4).  7 issue slots per
-// element (FMUL2 + 8 FFMA2 + FMUL2 per pair, FMNMX + FFMA.SAT per element) against 12 FMA-pipe + 2 MUFU for
-// gelu_erf_fast -- the sampler is power-capped (profiles/r2_power_ops.json), so instructions are time.
+// Phi to [0, 1], which is also the right limit for |x| > 4 (x Q(16) = +-0.49997 |x| / 4).
 // Error (fp32 evaluation, |x| <= 8): |abs| <= 1.1e-5 for |x| < 4, relative <= 5e-4 where |GELU| > 0.01, and GELU is
 // flushed to 0 below x = -4 (true value > -1.3e-4): all below the bf16 rounding of the stored result (2^-9).
 __device__ __forceinline__ void gelu_erf_poly2(float& a, float& b) {

@@ -15,7 +15,7 @@
 //             point and writes the vertex positions
 //   faces   : recount + intra-block scan; resolves the three cube edges of every triangle through the packed
 //             per-point word of the owning lattice point
-// The volume (28 MB at 192^3) stays in the 126 MB L2 between the passes; nothing else is materialised.
+// The volume (28 MB at 192^3) stays in the 50 MB L2 between the passes; nothing else is materialised.
 #include "common.cuh"
 #include "ln3_internal.h"
 #include "mc_tables.h"

@@ -1,4 +1,4 @@
-// Fused tri-plane volumetric renderer for sm_100a (fp32 SIMT, one warp per ray).
+// Fused tri-plane volumetric renderer for sm_90a (fp32 SIMT, one warp per ray).
 //
 // Replaces, for the Objaverse rendering preset (nsr/script_util.py:761-797), the whole of
 //   nsr/volumetric_rendering/renderer.py:133-307  ImportanceRenderer.forward
@@ -280,7 +280,7 @@ __device__ __noinline__ void eval_batch(const RenderParams& p, const BlockSmem& 
       // sampled_features.mean(1).  Exact path: IEEE division by 3 as torch's CPU mean (the oracle / goldens).
       // TF32 path: sum * (1/3) as torch's CUDA mean kernel computes it (MeanOps multiplies by the fp32 factor
       // 1/N) -- a last-ulp difference that the TF32 rounding of the MLP operand swallows; four IEEE divisions per
-      // lane here were ~10 % of the kernel's stall samples (profiles/r2_ncu_render_v3_tiles16.txt).
+      // lane here were ~10 % of the kernel's stall samples.
       if constexpr (TF32) {
         constexpr float kThird = 1.0f / 3.0f;
         ws.feat[sidx][c4 + 0] = ((f[0].x + f[1].x) + f[2].x) * kThird;

@@ -4,8 +4,8 @@
 context_dim=768, roll_out=True, vit_blk=TextCondDiTBlock)` is how the reference builds the
 denoiser (guided_diffusion/script_util.py:407-415); `.forward(x, timesteps, context)` returns the
 fp32 contiguous (B, 3*C, 32, 32) prediction (dit_trilatent.py:74-143).  The forward below is a
-fixed sequence of libln3b200 launches -- tcgen05 GEMMs with fused bias/GELU/gate-residual
-epilogues, the tcgen05 attention kernel, and three small SIMT kernels -- with fp32 residual
+fixed sequence of libln3b200 launches -- wgmma GEMMs with fused bias/GELU/gate-residual
+epilogues, the wgmma attention kernel, and three small SIMT kernels -- with fp32 residual
 stream and bf16 GEMM operands (the reference's bf16-autocast GPU path keeps the same split).
 """
 from __future__ import annotations

@@ -77,28 +77,8 @@ def gemm(a: torch.Tensor, w: torch.Tensor, bias: torch.Tensor | None = None, *,
         args.head_norm_w, args.head_norm_nsec = head_norm.data_ptr(), head_norm.shape[0]
         args.head_norm_sec_cols, args.head_norm_eps = head_norm_sec_cols, head_norm_eps
     args.act, args.out_kind = act, out_kind
-    if M >= 256 and os.environ.get("LN3_GEMM_STREAMK", "0") not in ("", "0"):   # opt-in stream-K tail
-        ws = _gemm_workspace(a.device)
-        args.workspace, args.workspace_bytes = ws.data_ptr(), ws.numel()
     _lib.check(_lib.lib().ln3_gemm_bf16(C.byref(args), _lib.current_stream()), "ln3_gemm_bf16")
     return out
-
-
-_GEMM_WS: dict = {}
-
-
-def _gemm_workspace(device: torch.device) -> torch.Tensor:
-    """Zero-initialised stream-K scratch (flags + partial accumulators), one per device; the kernel leaves
-    the flags zeroed.  The hot path issues its GEMMs on one stream at a time (they serialise); callers that
-    run GEMMs of this library concurrently on several streams must set LN3_GEMM_STREAMK=0."""
-    key = device.index if device.index is not None else torch.cuda.current_device()
-    ws = _GEMM_WS.get(key)
-    if ws is None:
-        if torch.cuda.is_current_stream_capturing():
-            raise RuntimeError("first GEMM of this device inside a CUDA-graph capture: run one forward before capturing")
-        ws = torch.zeros(_lib.lib().ln3_gemm_workspace_bytes(), device=device, dtype=torch.uint8)
-        _GEMM_WS[key] = ws
-    return ws
 
 
 def fmha(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, heads: int, *,

@@ -29,7 +29,7 @@ import importlib.util
 import sys
 import threading
 
-# reference module name -> mirror (one line per file of the hot path; DESIGN.md section 1)
+# reference module name -> mirror (one line per file of the hot path)
 MIRRORED = {
     "dit.dit_trilatent": "ln3diff_b200.dit.dit_trilatent",
     "dit.dit_i23d": "ln3diff_b200.dit.dit_i23d",

@@ -189,7 +189,7 @@ def kornia_resize_bicubic(x: torch.Tensor, size=(224, 224), antialias: bool = Tr
 
 
 def _patchify_gemm(img: torch.Tensor, w_packed: torch.Tensor, bias: Optional[torch.Tensor], patch: int) -> torch.Tensor:
-    """Conv2d(3, D, kernel = stride = patch) as one tcgen05 GEMM: (B*n*n, 3*p*p padded to a multiple of 64) x W^T.
+    """Conv2d(3, D, kernel = stride = patch) as one wgmma GEMM: (B*n*n, 3*p*p padded to a multiple of 64) x W^T.
     Non-overlapping patches: the unfold is a pure permute."""
     B, C, Hh, Ww = img.shape
     n = Hh // patch

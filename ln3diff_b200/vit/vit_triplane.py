@@ -6,7 +6,7 @@ Decode path (train_util_diffusion.py:188-206 -> nsr/script_util.py:243-259):
   vit_decode_backbone   (vit_triplane.py:996-1011, :2126-2132)  latent -> PatchEmbedTriplane -> DiT2
   vit_decode_postprocess (:1913-1977)                           tokens -> conv_sr -> (B, 96, 128, 128)
   triplane_decode       (:1013-1041)                            Triplane.forward(planes, c)
-Device work: tcgen05 GEMM / attention kernels for the 24 DiT2 blocks (per-token adaLN as one GEMM
+Device work: wgmma GEMM / attention kernels for the 24 DiT2 blocks (per-token adaLN as one GEMM
 per block), NHWC fp32 conv kernels for the SD decoder.  The DiT2 token stream is consumed by conv_in
 in place (tokens are NHWC) and conv_out writes the channels-last tri-plane the ray marcher reads."""
 from __future__ import annotations

@@ -11,7 +11,7 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA GPU (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA GPU (an H100, sm_90a; select with -m gpu)")
     # CPU oracle legs of the GPU tests: use the cores this process really has (cgroup quota), not the node's
     try:
         import torch

@@ -1,4 +1,4 @@
-"""CPU: the C-ABI library builds for sm_100a, loads, and exports every symbol include/*.h declares.
+"""CPU: the C-ABI library builds for sm_90a, loads, and exports every symbol include/*.h declares.
 No compute calls (there is no GPU here); compute entry points must fail loudly without one."""
 import ctypes
 import os
