@@ -127,6 +127,9 @@ int ln3_fmha_fwd(const ln3_fmha_args* args, void* stream);
  *          LN3_NORM_RMS  : x * rsqrt(mean(x^2) + eps) * weight        (dit/norm.py:27-40)
  *          LN3_NORM_NONE : identity (plain fp32 -> bf16 cast, optional activation LN3_ACT_*)
  * shift/scale NULL -> no modulation.  D must be a multiple of 128 and <= 2048.
+ * Alignment (LN3_EINVAL otherwise): x, out, shift, scale, shift_tab, scale_tab, weight, resid, resid_gate,
+ * resid_out_gate and resid_bcast 16-byte aligned; ldx, ldo, mod_ld, resid_ld, resid_gate_ld and
+ * resid_out_gate_ld multiples of 4, resid_bcast_ld a multiple of 8.
  */
 enum { LN3_NORM_NONE = 0, LN3_NORM_LAYER = 1, LN3_NORM_RMS = 2 };
 
@@ -191,7 +194,8 @@ int ln3_timestep_embedding(const float* t, int B, void* out_bf16, void* stream);
  * i.e. rearrange 'b (c n) h w -> (b n) c h w' + timm PatchEmbed + pos_embed
  * (dit/dit_trilatent.py:93-99).  x fp32 (B, 3*Cin, S, S) optionally pre-scaled per sample by
  * in_scale[b] (the denoiser's c_in, sgm/modules/diffusionmodules/denoiser.py:34-42);
- * weight fp32 (D, Cin, 2, 2); tokens fp32 (B, 3*(S/2)^2, D).
+ * weight fp32 (D, Cin, 2, 2); tokens fp32 (B, 3*(S/2)^2, D).  S even, 1 <= Cin <= 16.  Cin == 4 with D % 4 == 0
+ * takes the vectorised kernel only when weight, bias, pos_embed and tokens are 16-byte aligned.
  */
 typedef struct ln3_patch_embed_args {
   const float* x;
@@ -210,6 +214,8 @@ int ln3_patch_embed(const ln3_patch_embed_args* args, void* stream);
  * eps 1e-6) -> modulate(shift, scale (+ tables)) -> Linear(D -> 4*Cout) -> unpatchify ->
  * '(b n) c h w -> b (c n) h w' (dit/dit_trilatent.py:130-140), fp32 contiguous output
  * (B, 3*Cout, S, S).  shift/scale are [B, mod_ld] rows.
+ * LN3_EINVAL unless: S even, Cout > 0, D a multiple of 128 and <= 2048, mod_ld a multiple of 4, shift_tab and
+ * scale_tab both given or both NULL, and x, shift, scale, the tables and weight 16-byte aligned.
  */
 typedef struct ln3_final_layer_args {
   const float* x; /* tokens [B, 3*L, D] */
@@ -234,6 +240,7 @@ int ln3_final_layer(const ln3_final_layer_args* args, void* stream);
  *   DDPM p_sample (eps/x0/v, fixed variance)  guided_diffusion/gaussian_diffusion.py:273-546
  *   flow-matching Euler + CFG              transport/integrators.py:101-120, dit/dit_i23d.py:155-168
  * coef is [B, 4] = (a, w0, w1, s); m1 / noise may be NULL when their weight is unused.
+ * n_per_sample % 4 == 0; x, m0, m1, noise, coef and x_out 16-byte aligned (LN3_EINVAL otherwise).
  */
 typedef struct ln3_sampler_update_args {
   const float* x;

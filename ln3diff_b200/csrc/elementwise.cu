@@ -146,8 +146,8 @@ norm_modulate_kernel(const ln3_norm_modulate_args a) {
 
 // ---- 256-bit kernels (D % 256 == 0, 32-byte aligned rows: every DiT / DiT2 call) -------------------------
 // A lane owns NV8 chunks of 8 consecutive columns: the fp32 row moves as 256-bit accesses and the bf16 rows as
-// 128-bit accesses.  nm_row_body is the arithmetic of one row, shared by the two kernels below; same operations in
-// the same order per element as the float4 kernel above.
+// 128-bit accesses.  nm_row_body is the arithmetic of one row; same operations in the same order per element as
+// the float4 kernel above.
 //   v      the row of x (registers)
 //   rown   this row's own residual row resid[row] (bf16, one uint4 per chunk), meaningful iff nm_needs_own_row()
 __device__ __forceinline__ bool nm_outside(const ln3_norm_modulate_args& a, int row) {
@@ -286,13 +286,12 @@ __device__ __forceinline__ void nm_row_body(const ln3_norm_modulate_args& a, int
 }
 
 // Warp per row straight from global memory.  (A software-pipelined variant -- next row's loads issued before the
-// current row's arithmetic, 2 CTAs/SM at 128 registers -- measured slower: 36.9 vs 32.8 us; so did the shared-memory
-// staged kernel below.  Occupancy at <= 80 registers beats explicit prefetch here.)
+// current row's arithmetic, 2 CTAs/SM at 128 registers -- measured slower: 36.9 vs 32.8 us; so did a shared-memory
+// staged kernel fed by bulk copies, 48 vs 36 us.  Occupancy at <= 80 registers beats explicit prefetch here.)
 template <int NV8>
 __device__ __forceinline__ void nm_load_row(const ln3_norm_modulate_args& a, int row, int lane, float (&v)[NV8][8],
                                             uint4 (&rown)[NV8]) {
   const float* x = a.x + static_cast<long long>(row) * a.ldx;
-#pragma unroll
   if (c_nm_l2_hint) {
 #pragma unroll
     for (int i = 0; i < NV8; ++i) ldg256_na_el(x + (i * 32 + lane) * 8, v[i]);
@@ -330,109 +329,9 @@ norm_modulate_wide_kernel(const ln3_norm_modulate_args a) {
   }
 }
 
-// Staged variant for the big residual-stream passes (the three per DiT block: 150 MB each at DiT-L/2 B'=16).
-// The warp-per-row kernel keeps at most one row per warp in flight and stops loading while it reduces and stores
-// (ncu: 4.2-4.9 TB/s = 0.64-0.75 of the measured copy bandwidth, dram ~40 % busy).  Here a producer thread streams
-// the fp32 rows (and their bf16 residual rows) into a 4-stage shared-memory ring with 1-D bulk copies
-// (cp.async.bulk, byte-counted mbarriers), 8 rows per stage, so ~144 KB per SM is always in flight while 8 consumer
-// warps (one row each) run the unchanged arithmetic out of shared memory and store straight to global.
-static constexpr int kNmStages = 4, kNmRowsPerStage = 8;
-template <int NV8>
-constexpr int nm_stage_bytes() { return kNmRowsPerStage * NV8 * 256 * (4 + 2); }
-template <int NV8>
-constexpr int nm_staged_smem() { return kNmStages * nm_stage_bytes<NV8>() + 128; }
-
-template <int NV8>
-__global__ void __launch_bounds__((kNmRowsPerStage + 1) * 32, 1)
-norm_modulate_staged_kernel(const ln3_norm_modulate_args a) {
-  extern __shared__ __align__(128) uint8_t nm_smem[];
-  constexpr int D = NV8 * 256;
-  constexpr int kXBytes = D * 4, kRBytes = D * 2;
-  uint64_t* full = reinterpret_cast<uint64_t*>(nm_smem + kNmStages * nm_stage_bytes<NV8>());
-  uint64_t* empty = full + kNmStages;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < kNmStages; ++s) {
-      mbar_init(&full[s], 1);
-      mbar_init(&empty[s], kNmRowsPerStage);
-    }
-    fence_barrier_init();
-  }
-  __syncthreads();
-  pdl_launch_dependents();
-  pdl_wait();
-  const int n_groups = (a.rows + kNmRowsPerStage - 1) / kNmRowsPerStage;
-  // contiguous run of row groups per CTA: the per-sample modulation vectors (shift / scale / gate rows, shared by
-  // 768 consecutive token rows) stay hot in the 28 KB of L1 left beside the ring
-  const int gpb = (n_groups + static_cast<int>(gridDim.x) - 1) / static_cast<int>(gridDim.x);
-  const int g_begin = static_cast<int>(blockIdx.x) * gpb;
-  const int g_end = min(n_groups, g_begin + gpb);
-  if (warp == kNmRowsPerStage) {
-    // ---- producer: one lane issues the bulk copies of a whole stage
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int g = g_begin; g < g_end; ++g) {
-        mbar_wait(&empty[stage], phase ^ 1);
-        uint8_t* sx = nm_smem + stage * nm_stage_bytes<NV8>();
-        uint8_t* sr = sx + kNmRowsPerStage * kXBytes;
-        const int row0 = g * kNmRowsPerStage;
-        const int nrows = min(kNmRowsPerStage, a.rows - row0);
-        // contiguous rows (the usual case: x and resid are dense [rows, D] buffers) move as ONE bulk copy per
-        // operand and stage -- a bulk-copy instruction costs hundreds of issue cycles on the producer thread, and
-        // sixteen 2-4 KB copies per stage made the producer the bottleneck (2.4 TB/s)
-        int n_own = 0;
-        for (int r = 0; r < nrows; ++r) n_own += nm_needs_own_row(a, row0 + r) ? 1 : 0;
-        mbar_arrive_expect_tx(&full[stage], nrows * kXBytes + n_own * kRBytes);
-        if (a.ldx == D) {
-          bulk_load_1d(sx, a.x + static_cast<long long>(row0) * a.ldx, nrows * kXBytes, &full[stage]);
-        } else {
-          for (int r = 0; r < nrows; ++r)
-            bulk_load_1d(sx + r * kXBytes, a.x + static_cast<long long>(row0 + r) * a.ldx, kXBytes, &full[stage]);
-        }
-        if (n_own == nrows && a.resid_ld == D) {
-          bulk_load_1d(sr, reinterpret_cast<const __nv_bfloat16*>(a.resid) + static_cast<long long>(row0) * a.resid_ld,
-                       nrows * kRBytes, &full[stage]);
-        } else if (n_own > 0) {
-          for (int r = 0; r < nrows; ++r)
-            if (nm_needs_own_row(a, row0 + r))
-              bulk_load_1d(sr + r * kRBytes,
-                           reinterpret_cast<const __nv_bfloat16*>(a.resid) + static_cast<long long>(row0 + r) * a.resid_ld,
-                           kRBytes, &full[stage]);
-        }
-        if (++stage == kNmStages) stage = 0, phase ^= 1;
-      }
-    }
-    return;
-  }
-  // ---- consumers: warp w owns row w of every stage
-  int stage = 0;
-  uint32_t phase = 0;
-  for (int g = g_begin; g < g_end; ++g) {
-    const int row = g * kNmRowsPerStage + warp;
-    mbar_wait(&full[stage], phase);
-    float v[NV8][8];
-    uint4 rown[NV8];
-    const bool live = row < a.rows;
-    if (live) {
-      const uint8_t* sx = nm_smem + stage * nm_stage_bytes<NV8>() + warp * kXBytes;
-      const uint8_t* sr = nm_smem + stage * nm_stage_bytes<NV8>() + kNmRowsPerStage * kXBytes + warp * kRBytes;
-      const bool own = nm_needs_own_row(a, row);
-#pragma unroll
-      for (int i = 0; i < NV8; ++i) {
-        const float4 lo = *reinterpret_cast<const float4*>(sx + (i * 32 + lane) * 32);
-        const float4 hi = *reinterpret_cast<const float4*>(sx + (i * 32 + lane) * 32 + 16);
-        v[i][0] = lo.x, v[i][1] = lo.y, v[i][2] = lo.z, v[i][3] = lo.w;
-        v[i][4] = hi.x, v[i][5] = hi.y, v[i][6] = hi.z, v[i][7] = hi.w;
-        rown[i] = own ? *reinterpret_cast<const uint4*>(sr + (i * 32 + lane) * 16) : make_uint4(0, 0, 0, 0);
-      }
-    }
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&empty[stage]);   // the row is in registers: the producer may refill the slot
-    if (live) nm_row_body<NV8>(a, row, lane, v, rown);
-    if (++stage == kNmStages) stage = 0, phase ^= 1;
-  }
-}
+// Every pointer the glue kernels read or write with 128-bit (or 64-bit) accesses must be 16-byte aligned: a
+// column-offset view such as mod[:, 1:1+D] would otherwise pass the shape checks and issue misaligned loads.
+static bool misaligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) != 0; }
 
 int norm_modulate(const ln3_norm_modulate_args* a, cudaStream_t stream) {
   if (a->rows <= 0) return LN3_OK;
@@ -447,12 +346,17 @@ int norm_modulate(const ln3_norm_modulate_args* a, cudaStream_t stream) {
   if (a->ldx % 4 || a->ldo % 4 || (a->shift && a->mod_ld % 4))
     return set_error(LN3_EINVAL, "norm_modulate: leading dimensions must be multiples of 4");
   if (a->out == nullptr && a->resid == nullptr) return set_error(LN3_EINVAL, "norm_modulate: out is NULL");
+  // out and resid need only 8 bytes in the float4 kernel and 16 in the 256-bit one: one rule, the stricter
+  if (misaligned16(a->x) || misaligned16(a->out) || misaligned16(a->shift) || misaligned16(a->scale) ||
+      misaligned16(a->shift_tab) || misaligned16(a->scale_tab) || misaligned16(a->weight) || misaligned16(a->resid) ||
+      misaligned16(a->resid_gate) || misaligned16(a->resid_bcast) || misaligned16(a->resid_out_gate))
+    return set_error(LN3_EINVAL, "norm_modulate: x, out, shift, scale, tables, weight, resid, resid_bcast and gates must be 16-byte aligned");
   if (a->resid != nullptr) {
     if (a->resid_ld % 4) return set_error(LN3_EINVAL, "norm_modulate: resid_ld must be a multiple of 4");
     if (a->resid_gate != nullptr && (a->resid_gate_rows <= 0 || a->resid_gate_ld % 4))
       return set_error(LN3_EINVAL, "norm_modulate: bad resid_gate_rows / resid_gate_ld");
     if (a->resid_bcast != nullptr &&
-        (a->resid_bcast_rows <= 0 || a->resid_bcast_ld % 8 || (reinterpret_cast<uintptr_t>(a->resid_bcast) & 15) ||
+        (a->resid_bcast_rows <= 0 || a->resid_bcast_ld % 8 ||
          a->resid_row_begin < 0 || a->resid_row_end < a->resid_row_begin || a->resid_row_end > a->rows))
       return set_error(LN3_EINVAL, "norm_modulate: bad resid_bcast arguments");
     if (a->resid_out_gate != nullptr &&
@@ -469,10 +373,6 @@ int norm_modulate(const ln3_norm_modulate_args* a, cudaStream_t stream) {
   const bool wide = wide_enabled && a->D % 256 == 0 && a->D <= 1536 && a->ldx % 8 == 0 && a->ldo % 8 == 0 &&
                     (reinterpret_cast<uintptr_t>(a->x) & 31) == 0 && (a->out == nullptr || (reinterpret_cast<uintptr_t>(a->out) & 15) == 0) &&
                     (a->resid == nullptr || (a->resid_ld % 8 == 0 && (reinterpret_cast<uintptr_t>(a->resid) & 15) == 0));
-  // opt-in (LN3_NORM_STAGED=1): shared-memory staged kernel for the big residual-stream passes.  Measured slower
-  // than the warp-per-row kernel (48 vs 36 us for LN + residual at DiT-L/2 B'=16): with the ring taking 196 KB the
-  // CTA has 8 consumer warps and 28 KB of L1, and the per-row arithmetic (two reductions, the modulation-vector
-  // loads) then bounds the pass, not the loads.
   {  // LN3_RESID_L2=1: evict_last hints on the residual stream (uploaded once per device)
     static DeviceOnce l2_once;
     if (int rc = l2_once.run([] {
@@ -481,33 +381,6 @@ int norm_modulate(const ln3_norm_modulate_args* a, cudaStream_t stream) {
           return e == cudaSuccess ? LN3_OK : set_error(LN3_ECUDA, "norm_modulate: constant upload: %s", cudaGetErrorString(e));
         }))
       return rc;
-  }
-  static const bool staged_enabled = getenv("LN3_NORM_STAGED") && atoi(getenv("LN3_NORM_STAGED")) != 0;
-  if (wide && staged_enabled && a->D <= 1024 && a->rows >= 2048 && (a->ldx * 4) % 16 == 0 &&
-      (a->resid == nullptr || (a->resid_ld * 2) % 16 == 0)) {
-    const int sms = device_sm_count();
-    const int n_groups = (a->rows + kNmRowsPerStage - 1) / kNmRowsPerStage;
-    const dim3 sgrid(n_groups < sms ? n_groups : sms), sblock((kNmRowsPerStage + 1) * 32);
-    static DeviceOnce once;
-    if (int rc = once.run([] {
-          cudaError_t e = cudaFuncSetAttribute(norm_modulate_staged_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, nm_staged_smem<1>());
-          if (e == cudaSuccess) e = cudaFuncSetAttribute(norm_modulate_staged_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, nm_staged_smem<2>());
-          if (e == cudaSuccess) e = cudaFuncSetAttribute(norm_modulate_staged_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, nm_staged_smem<3>());
-          if (e == cudaSuccess) e = cudaFuncSetAttribute(norm_modulate_staged_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, nm_staged_smem<4>());
-          return e == cudaSuccess ? LN3_OK : set_error(LN3_ECUDA, "norm_modulate: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
-        }))
-      return rc;
-    cudaError_t le = cudaSuccess;
-    switch (a->D / 256) {
-      case 1: le = launch_pdl(norm_modulate_staged_kernel<1>, sgrid, sblock, nm_staged_smem<1>(), stream, *a); break;
-      case 2: le = launch_pdl(norm_modulate_staged_kernel<2>, sgrid, sblock, nm_staged_smem<2>(), stream, *a); break;
-      case 3: le = launch_pdl(norm_modulate_staged_kernel<3>, sgrid, sblock, nm_staged_smem<3>(), stream, *a); break;
-      default: le = launch_pdl(norm_modulate_staged_kernel<4>, sgrid, sblock, nm_staged_smem<4>(), stream, *a); break;
-    }
-    cudaError_t e = le != cudaSuccess ? le : cudaGetLastError();
-    if (e != cudaSuccess) return set_error(LN3_ECUDA, "norm_modulate launch: %s", cudaGetErrorString(e));
-    count_launch();
-    return LN3_OK;
   }
   if (wide) {
     cudaError_t le = cudaSuccess;
@@ -660,7 +533,9 @@ int patch_embed(const ln3_patch_embed_args* a, cudaStream_t stream) {
   if (a->S % 2 || a->Cin <= 0 || a->Cin > 16 || a->D <= 0)
     return set_error(LN3_EINVAL, "patch_embed: need even S, 1 <= Cin <= 16");
   const int L = (a->S / 2) * (a->S / 2);
-  if (a->Cin == 4 && a->D % 4 == 0)
+  // the k16 kernel moves weight, bias, pos_embed and tokens as float4; the generic kernel uses scalar accesses
+  if (a->Cin == 4 && a->D % 4 == 0 && !misaligned16(a->weight) && !misaligned16(a->bias) &&
+      !misaligned16(a->pos_embed) && !misaligned16(a->tokens))
     patch_embed_k16_kernel<<<(a->B * 3 * L + kPeTok - 1) / kPeTok, 256, 0, stream>>>(*a);
   else
     patch_embed_kernel<<<a->B * 3 * L, 256, 0, stream>>>(*a);
@@ -836,6 +711,15 @@ int final_layer(const ln3_final_layer_args* a, cudaStream_t stream) {
   if (a->D % 128 != 0 || a->D > 2048) return set_error(LN3_EINVAL, "final_layer: bad D=%d", a->D);
   if (a->shift == nullptr || a->scale == nullptr)
     return set_error(LN3_EINVAL, "final_layer: shift/scale required");
+  // odd S would leave the last output row and column unwritten (tokens cover 2x2 patches)
+  if (a->S <= 0 || a->S % 2 || a->Cout <= 0)
+    return set_error(LN3_EINVAL, "final_layer: need even S > 0 and Cout > 0 (S=%d, Cout=%d)", a->S, a->Cout);
+  if (a->mod_ld % 4) return set_error(LN3_EINVAL, "final_layer: mod_ld must be a multiple of 4");
+  if ((a->shift_tab == nullptr) != (a->scale_tab == nullptr))
+    return set_error(LN3_EINVAL, "final_layer: shift_tab and scale_tab must be given together");
+  if (misaligned16(a->x) || misaligned16(a->shift) || misaligned16(a->scale) || misaligned16(a->shift_tab) ||
+      misaligned16(a->scale_tab) || misaligned16(a->weight))
+    return set_error(LN3_EINVAL, "final_layer: x, shift, scale, tables and weight must be 16-byte aligned");
   const int L = (a->S / 2) * (a->S / 2);
   const int toks = a->B * 3 * L;
   dim3 grid((toks + 3) / 4), block(128);
@@ -896,6 +780,9 @@ int sampler_affine_update(const ln3_sampler_update_args* a, cudaStream_t stream)
   if (a->B <= 0 || a->n_per_sample <= 0) return LN3_OK;
   if (a->n_per_sample % 4) return set_error(LN3_EINVAL, "sampler_update: n_per_sample % 4 != 0");
   if (!a->x || !a->m0 || !a->coef || !a->x_out) return set_error(LN3_EINVAL, "sampler_update: null pointer");
+  if (misaligned16(a->x) || misaligned16(a->m0) || misaligned16(a->m1) || misaligned16(a->noise) ||
+      misaligned16(a->x_out) || misaligned16(a->coef))
+    return set_error(LN3_EINVAL, "sampler_update: x, m0, m1, noise, x_out and coef must be 16-byte aligned");
   const long long n4 = a->n_per_sample / 4;
   int gx = static_cast<int>((n4 + 255) / 256);
   if (gx > 1024) gx = 1024;

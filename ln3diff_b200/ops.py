@@ -267,7 +267,12 @@ def final_layer(x: torch.Tensor, shift: torch.Tensor, scale: torch.Tensor, weigh
     if bias is not None:
         _cuda(bias, "bias", torch.float32)
         a.bias = bias.data_ptr()
+    _req((shift_tab is None) == (scale_tab is None), "shift_tab and scale_tab must be given together")
     if shift_tab is not None:
+        _cuda(shift_tab, "shift_tab", torch.float32)
+        _cuda(scale_tab, "scale_tab", torch.float32)
+        _req(shift_tab.shape == (D,) and scale_tab.shape == (D,) and shift_tab.is_contiguous()
+             and scale_tab.is_contiguous(), "tables must be contiguous (D,)")
         a.shift_tab, a.scale_tab = shift_tab.data_ptr(), scale_tab.data_ptr()
     a.B, a.S, a.D, a.Cout, a.mod_ld = B, S, D, Cout, shift.stride(0)
     _lib.check(_lib.lib().ln3_final_layer(C.byref(a), _lib.current_stream()), "ln3_final_layer")
