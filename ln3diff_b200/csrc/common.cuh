@@ -72,6 +72,15 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   }
 }
 
+// mbar_wait without the diagnostic printf, for loops that keep a wgmma group in flight across the wait: a function
+// call there (vprintf) makes ptxas serialise every wgmma of the kernel (C7510).  A timeout still traps.
+__device__ __forceinline__ void mbar_wait_silent(uint64_t* bar, uint32_t parity) {
+  uint32_t spins = 0;
+  while (!mbar_try_wait(bar, parity)) {
+    if (++spins == (1u << 26)) __trap();
+  }
+}
+
 // try_wait with an explicit suspend-time hint (ns): the thread may sleep in hardware until the phase completes or the
 // time limit passes, instead of returning after the (short, implementation-defined) default slice -- a waiting warp
 // then stops feeding try_wait / branch pairs into the issue slots and the MIO queue of the math warps it shares a
@@ -128,6 +137,12 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m
 }
 
 // smem -> global tile store (bulk async group); rows / columns outside the tensor are clipped.
+__device__ __forceinline__ void tma_store_2d(const void* smem_src, const CUtensorMap* m, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
+                   reinterpret_cast<uint64_t>(m)),
+               "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
+               : "memory");
+}
 __device__ __forceinline__ void tma_store_3d(const void* smem_src, const CUtensorMap* m, int c0, int c1, int c2) {
   asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(
                    reinterpret_cast<uint64_t>(m)),
@@ -217,6 +232,12 @@ __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
 __device__ __forceinline__ void named_bar_arrive(int id, int nthreads) {
   asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
+// Move registers between the warpgroups of a CTA (every thread of the warpgroup executes it): a warpgroup that
+// only issues TMA gives registers back, the MMA warpgroups take them.
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 // fp32 pairs held in one 64-bit value; fma2 evaluates both lanes with scalar FMAs (same rounding as the
 // packed form: one fma.rn per lane).
 __device__ __forceinline__ uint64_t pk2(float lo, float hi) {
