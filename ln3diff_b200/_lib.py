@@ -70,6 +70,13 @@ class PatchEmbedArgs(C.Structure):
     ]
 
 
+class PluckerPatchifyArgs(C.Structure):
+    _fields_ = [
+        ("image", C.c_void_p), ("cams", C.c_void_p), ("out", C.c_void_p),
+        ("N", C.c_int), ("ldo", C.c_longlong),
+    ]
+
+
 class FinalLayerArgs(C.Structure):
     _fields_ = [
         ("x", C.c_void_p), ("shift", C.c_void_p), ("scale", C.c_void_p), ("shift_tab", C.c_void_p),

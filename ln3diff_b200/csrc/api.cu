@@ -132,6 +132,10 @@ int ln3_patch_embed(const ln3_patch_embed_args* args, void* stream) {
   if (!args) return set_error(LN3_EINVAL, "patch_embed: null args");
   return patch_embed(args, static_cast<cudaStream_t>(stream));
 }
+int ln3_plucker_patchify(const ln3_plucker_patchify_args* args, void* stream) {
+  if (!args) return set_error(LN3_EINVAL, "plucker_patchify: null args");
+  return plucker_patchify(args, static_cast<cudaStream_t>(stream));
+}
 int ln3_final_layer(const ln3_final_layer_args* args, void* stream) {
   if (!args) return set_error(LN3_EINVAL, "final_layer: null args");
   return final_layer(args, static_cast<cudaStream_t>(stream));

@@ -70,6 +70,7 @@ int fmha_fwd(const ln3_fmha_args* a, cudaStream_t stream);
 int norm_modulate(const ln3_norm_modulate_args* a, cudaStream_t stream);
 int timestep_embedding(const float* t, int B, void* out_bf16, cudaStream_t stream);
 int patch_embed(const ln3_patch_embed_args* a, cudaStream_t stream);
+int plucker_patchify(const ln3_plucker_patchify_args* a, cudaStream_t stream);
 int final_layer(const ln3_final_layer_args* a, cudaStream_t stream);
 int sampler_affine_update(const ln3_sampler_update_args* a, cudaStream_t stream);
 size_t render_workspace_bytes(int V, int M, int group_size);

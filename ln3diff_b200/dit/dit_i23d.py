@@ -43,8 +43,14 @@ class ImageCondDiTBlockPixelArtRMSNorm(nn.Module):
         self.adaLN_modulation = None
 
 
+class ImageCondDiTBlockPixelArtRMSNormNoClip(ImageCondDiTBlockPixelArtRMSNorm):
+    """reference dit/dit_models_xformers.py:541-601,621-635: the same parameters (attention_y_norm included, unused);
+    its forward runs self-attention over the latent tokens only and cross-attends the multi-view DINO tokens."""
+
+
 class DiT_I23D_PixelArt(PixArtGraphMixin, nn.Module):
     _ln3_fused_in_scale = False
+    _vit_blk = ImageCondDiTBlockPixelArtRMSNorm
 
     def __init__(self, input_size=32, patch_size=2, in_channels=4, hidden_size=1152, depth=28, num_heads=16,
                  mlp_ratio=4, class_dropout_prob=0.1, num_classes=1000, learn_sigma=True, mixing_logit_init=-3,
@@ -54,8 +60,8 @@ class DiT_I23D_PixelArt(PixArtGraphMixin, nn.Module):
         assert roll_out
         if patch_size != 2 or hidden_size // num_heads != 64:
             raise NotImplementedError("libln3b200 implements patch_size=2, head_dim=64")
-        if vit_blk is not ImageCondDiTBlockPixelArtRMSNorm:
-            raise NotImplementedError("release I23D uses ImageCondDiTBlockPixelArtRMSNorm")
+        if vit_blk is not self._vit_blk:
+            raise NotImplementedError(f"{type(self).__name__} uses {self._vit_blk.__name__}")
         assert num_classes == 0
         self.plane_n, self.depth, self.mlp_ratio = 3, depth, mlp_ratio
         self.learn_sigma, self.in_channels = learn_sigma, in_channels
@@ -112,15 +118,11 @@ class DiT_I23D_PixelArt(PixArtGraphMixin, nn.Module):
         P = dict(t0_w=bf(self.t_embedder.mlp[0].weight), t0_b=f32(self.t_embedder.mlp[0].bias),
                  t2_w=bf(self.t_embedder.mlp[2].weight), t2_b=f32(self.t_embedder.mlp[2].bias),
                  ada_w=bf(self.adaLN_modulation[1].weight), ada_b=f32(self.adaLN_modulation[1].bias),
-                 cap_ln_w=f32(self.cap_embedder[0].weight), cap_ln_b=f32(self.cap_embedder[0].bias),
-                 cap_w=bf(self.cap_embedder[1].weight), cap_b=f32(self.cap_embedder[1].bias),
-                 ynorm_w=f32(self.attention_y_norm.weight),
-                 d1_w=bf(self.dino_proj.y_proj.fc1.weight), d1_b=f32(self.dino_proj.y_proj.fc1.bias),
-                 d2_w=bf(self.dino_proj.y_proj.fc2.weight), d2_b=f32(self.dino_proj.y_proj.fc2.bias),
                  pe_w=f32(self.x_embedder.proj.weight), pe_b=f32(self.x_embedder.proj.bias), pos=f32(self.pos_embed),
                  fin_w=f32(self.final_layer.linear.weight), fin_b=f32(self.final_layer.linear.bias),
                  fin_tab=f32(self.final_layer.scale_shift_table),
-                 tables=f32(torch.stack([b.scale_shift_table.detach().reshape(-1) for b in self.blocks], 0)))
+                 tables=f32(torch.stack([b.scale_shift_table.detach().reshape(-1) for b in self.blocks], 0)),
+                 **self._prepare_context_weights(bf, f32))
         blocks = []
         for b in self.blocks:
             qkv_w, qkv_b = b.attn.qkv.weight.detach(), b.attn.qkv.bias.detach()
@@ -128,8 +130,7 @@ class DiT_I23D_PixelArt(PixArtGraphMixin, nn.Module):
                 n1_w=f32(b.norm1.weight), n2_w=f32(b.norm2.weight),
                 qkv_w=bf(qkv_w), qkv_b=f32(qkv_b),
                 qk_norm=f32(torch.stack([b.attn.q_norm.weight.detach(), b.attn.k_norm.weight.detach()], 0)),
-                kv_w=bf(qkv_w[D:]), kv_b=f32(qkv_b[D:]),                       # K|V rows for the DINO tokens
-                k_norm=f32(b.attn.k_norm.weight.detach()[None]),
+                **self._prepare_block_context_weights(b, bf, f32),
                 proj_w=bf(b.attn.proj.weight), proj_b=f32(b.attn.proj.bias),
                 cq_w=bf(b.cross_attn.to_q.weight), cq_norm=f32(b.cross_attn.q_norm.weight.detach()[None]),
                 ckv_w=bf(torch.cat([b.cross_attn.to_k.weight.detach(), b.cross_attn.to_v.weight.detach()], 0)),
@@ -141,6 +142,20 @@ class DiT_I23D_PixelArt(PixArtGraphMixin, nn.Module):
         self._invalidate()
         self._prep = P
         return P
+
+    def _prepare_context_weights(self, bf, f32) -> dict:
+        """Model-level weights of the conditioning: cap_embedder, attention_y_norm, dino_proj."""
+        return dict(cap_ln_w=f32(self.cap_embedder[0].weight), cap_ln_b=f32(self.cap_embedder[0].bias),
+                    cap_w=bf(self.cap_embedder[1].weight), cap_b=f32(self.cap_embedder[1].bias),
+                    ynorm_w=f32(self.attention_y_norm.weight),
+                    d1_w=bf(self.dino_proj.y_proj.fc1.weight), d1_b=f32(self.dino_proj.y_proj.fc1.bias),
+                    d2_w=bf(self.dino_proj.y_proj.fc2.weight), d2_b=f32(self.dino_proj.y_proj.fc2.bias))
+
+    def _prepare_block_context_weights(self, b, bf, f32) -> dict:
+        """Per-block K|V rows of the qkv projection (and the k_norm) for the DINO tokens of self-attention."""
+        D = self.embed_dim
+        return dict(kv_w=bf(b.attn.qkv.weight[D:]), kv_b=f32(b.attn.qkv.bias[D:]),
+                    k_norm=f32(b.attn.k_norm.weight.detach()[None]))
 
     @torch.no_grad()
     def _context(self, context):
@@ -207,19 +222,81 @@ class DiT_I23D_PixelArt(PixArtGraphMixin, nn.Module):
         return torch.cat([half, half], dim=0)
 
 
-def _mk(depth, hidden, heads):
+class DiT_I23D_PixelArt_MVCond_noClip(DiT_I23D_PixelArt):
+    """Mirror of reference dit/dit_i23d.py:392-492, the multi-view denoiser of the MV23D release
+    (`DiT-PixArt-MV-L/2`, shell_scripts/final_release/inference/sample_obajverse_mv23d_dit.sh): the I23D PixArt
+    model without dino_proj / clip_spatial_proj / cap_embedder, so t = t_embedder(timesteps) alone, and
+    `ImageCondDiTBlockPixelArtRMSNormNoClip` blocks: self-attention over the 768 latent tokens only and
+    cross-attention to the flattened multi-view DINO tokens context['concat'] (B, V, 256, C) -> (B, V*256, C), with
+    no attention_y_norm.  Same launch sequence as DiT_I23D_PixelArt (`pixart_forward`): the pooled embedding is a
+    zero row, there is no second self-attention K/V source, and every layer's cross-attention K|V of the DINO tokens
+    is computed once per condition batch."""
+    _vit_blk = ImageCondDiTBlockPixelArtRMSNormNoClip
+
+    def __init__(self, input_size=32, patch_size=2, in_channels=4, hidden_size=1152, depth=28, num_heads=16,
+                 mlp_ratio=4, class_dropout_prob=0.1, num_classes=1000, learn_sigma=True, mixing_logit_init=-3,
+                 mixed_prediction=True, context_dim=False, pooling_ctx_dim=768, roll_out=False, vit_blk=None,
+                 final_layer_blk=None):
+        # the reference passes ImageCondDiTBlockPixelArtRMSNormNoClip whatever vit_blk says (:413-420)
+        super().__init__(input_size, patch_size, in_channels, hidden_size, depth, num_heads, mlp_ratio,
+                         class_dropout_prob, num_classes, learn_sigma, mixing_logit_init, mixed_prediction, context_dim,
+                         pooling_ctx_dim, roll_out, ImageCondDiTBlockPixelArtRMSNormNoClip, final_layer_blk)
+        del self.dino_proj
+        del self.clip_spatial_proj, self.cap_embedder
+
+    def _prepare_context_weights(self, bf, f32) -> dict:
+        return {}
+
+    def _prepare_block_context_weights(self, b, bf, f32) -> dict:
+        return {}
+
+    @torch.no_grad()
+    def _context(self, context):
+        """Step-invariant conditioning, once per condition batch: every layer's cross-attention K|V of the
+        flattened DINO tokens (one GEMM per layer with the k_norm head epilogue)."""
+        ca0 = context["concat"]
+        hit = self._ctx_cache.get(ca0)
+        if hit is not None:
+            return hit
+        P, D = self._prep, self.embed_dim
+        B = ca0.shape[0]
+        tok = ca0.reshape(B, -1, ca0.shape[-1]).float()               # 'b v l c -> b (v l) c'
+        Lc = tok.shape[1]
+        dev = tok.device
+        st = self._static((B, Lc), lambda: dict(
+            cls=torch.zeros(B, D, device=dev, dtype=torch.float32),  # no pooled embedding: t + 0 == t
+            ckv=torch.empty(self.depth, B, Lc, 2 * D, device=dev, dtype=torch.bfloat16),
+            oc=torch.empty(self.depth, B, D, device=dev, dtype=torch.bfloat16)))
+        ctx = ops.norm_modulate(tok.reshape(B * Lc, -1).contiguous(), norm=NORM_NONE)   # bf16 GEMM operand
+        ckv = st["ckv"]
+        for l, W in enumerate(P["blocks"]):
+            ops.gemm(ctx, W["ckv_w"], out=ckv[l].view(B * Lc, 2 * D), head_norm=W["ck_norm"], head_norm_sec_cols=D)
+        out = dict(cls=st["cls"], ckv=ckv, rows=(0, B), oconst=None)
+        # the all-zero unconditional half: closed-form cross-attention (see DiT_I23D_PixelArt._context)
+        rows = _attention_rows(tok)
+        if rows is not None:
+            oc = st["oc"]
+            for l, W in enumerate(P["blocks"]):
+                ops.gemm(ckv[l][:, 0, D:].contiguous(), W["co_w"], W["co_b"], out=oc[l])
+            out.update(rows=rows, oconst=oc)
+        return self._ctx_cache.put((ca0,), out)
+
+
+def _mk(depth, hidden, heads, cls=DiT_I23D_PixelArt):
     def f(**kwargs):
-        return DiT_I23D_PixelArt(depth=depth, hidden_size=hidden, patch_size=2, num_heads=heads, **kwargs)
+        return cls(depth=depth, hidden_size=hidden, patch_size=2, num_heads=heads, **kwargs)
     return f
 
 
 def _unbuilt(name):
     def f(**kwargs):
-        raise NotImplementedError(f"{name}: not implemented in ln3diff_b200 (release I23D = DiT-PixArt-L/2)")
+        raise NotImplementedError(f"{name}: not implemented in ln3diff_b200 (release I23D = DiT-PixArt-L/2, "
+                                  f"release MV23D = DiT-PixArt-MV-L/2)")
     return f
 
 
-# reference dit/dit_i23d.py:685-697
+# reference dit/dit_i23d.py:685-697 ('DiT-PixArt-MV-L/2' -> DiT_L_Pixelart_MV_2_noclip, :651-656,693)
 DiT_models = {"DiT-PixArt-L/2": _mk(24, 1024, 16), "DiT-PixArt-B/2": _mk(12, 768, 12),
+              "DiT-PixArt-MV-L/2": _mk(24, 1024, 16, DiT_I23D_PixelArt_MVCond_noClip),
               **{k: _unbuilt(k) for k in ("DiT-XL/2", "DiT-L/2", "DiT-B/2", "DiT-B/1", "DiT-PixArt-MV-XL/2",
-                                         "DiT-PixArt-MV-L/2", "DiT-PixArt-MV-PCD-L", "DiT-PixArt-MV-B/2")}}
+                                         "DiT-PixArt-MV-PCD-L", "DiT-PixArt-MV-B/2")}}

@@ -243,6 +243,36 @@ def patch_embed(x: torch.Tensor, weight: torch.Tensor, bias: torch.Tensor | None
     return out
 
 
+PLUCKER_COLS = 9 * 14 * 14          # RGB + 6 Plücker channels of a 14x14 patch
+
+
+def plucker_patchify(image: torch.Tensor, cams: torch.Tensor, out: torch.Tensor | None = None,
+                     ldo: int = 1792) -> torch.Tensor:
+    """image fp32 (N,3,224,224) pre-processed views, cams fp32 (N,25) -> the bf16 patch operand (N*256, ldo) of the
+    9-channel 14x14 patch embedding: RGB | o x d | d per pixel in Conv2d.weight.reshape(D, -1) column order,
+    columns [1764, ldo) zero (FrozenDinov2ImageEmbedderMVPlucker's gen_rays / get_plucker_ray / cat / cast)."""
+    _cuda(image, "image", torch.float32)
+    _cuda(cams, "cams", torch.float32)
+    _req(image.dim() == 4 and image.shape[1:] == (3, 224, 224) and image.is_contiguous(),
+         "image must be contiguous (N,3,224,224)")
+    N = image.shape[0]
+    _req(cams.shape == (N, 25) and cams.is_contiguous(), "cams must be contiguous (N,25)")
+    if out is None:
+        out = torch.empty((N * 256, ldo), device=image.device, dtype=torch.bfloat16)
+    _cuda(out, "out", torch.bfloat16)
+    _req(out.dim() == 2 and out.shape[0] == N * 256 and out.shape[1] >= PLUCKER_COLS and out.stride(1) == 1,
+         "out must be (N*256, >= 1764) with unit inner stride")
+    # the kernel writes whole rows of `ldo` elements (zero padding up to the pitch)
+    _req(out.shape[1] % 8 == 0 and (N == 0 or out.stride(0) == out.shape[1]),
+         "out rows must be a multiple of 8 elements wide, with the row pitch equal to the width")
+    for nm, t_ in (("image", image), ("cams", cams), ("out", out)):
+        _req(t_.data_ptr() % 16 == 0, f"{nm} must be 16-byte aligned")
+    a = _lib.PluckerPatchifyArgs()
+    a.image, a.cams, a.out, a.N, a.ldo = image.data_ptr(), cams.data_ptr(), out.data_ptr(), N, out.shape[1]
+    _lib.check(_lib.lib().ln3_plucker_patchify(C.byref(a), _lib.current_stream()), "ln3_plucker_patchify")
+    return out
+
+
 def final_layer(x: torch.Tensor, shift: torch.Tensor, scale: torch.Tensor, weight: torch.Tensor,
                 bias: torch.Tensor | None, S: int, *, shift_tab: torch.Tensor | None = None,
                 scale_tab: torch.Tensor | None = None, out: torch.Tensor | None = None) -> torch.Tensor:

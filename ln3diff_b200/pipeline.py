@@ -175,6 +175,78 @@ def text_to_3d(conditioner, model, decoder, prompt, cameras, num_samples: int = 
     return generate_t23d(model, decoder, randn, c, uc, cameras, num_steps, scale, resolution)
 
 
+@torch.no_grad()
+def sample_flow(model, c: dict, uc: dict, num_samples: int, seed: int = 42, num_steps: int = 250,
+                cfg_scale: float = 4.0, sampling_method: str = "dopri5", dtype=torch.float32) -> torch.Tensor:
+    """`FlowMatchingEngine.sample` (nsr/lsgm/flow_matching_trainer.py:509-551) for the image-conditioned denoisers
+    (I23D 'img', MV23D 'img-c'): global `torch.manual_seed(seed)` -- which also seeds the CUDA generators that the
+    renderer's noise draws use afterwards -- then a CPU `randn(num_samples, 12, 32, 32)`, the CFG batch
+    cat((cond, uc)) per conditioning key and cat([zs, zs]), `Sampler(create_transport(snr_type='lognorm'))
+    .sample_ode(num_steps=..., sampling_method=...)` around `model.forward_with_cfg`, and `[-1].chunk(2)[0]`.
+
+    Engine dtype: as on the existing I23D path, the ODE state and the context are carried in fp32 and the denoiser
+    rounds its GEMM operands to bf16 itself.  The engine's `.to(self.dtype)` casts of the noise and the context
+    (bf16 under `use_amp`) are applied as roundings to `dtype`; the default float32 leaves them exact.
+    Returns the denoised latents (num_samples, 12, 32, 32) fp32."""
+    from .transport import Sampler, create_transport
+    dev = next(model.parameters()).device
+    if dev.type != "cuda":
+        raise RuntimeError("sample_flow runs on CUDA only (no CPU fallback)")
+    torch.manual_seed(seed)
+    C = 3 * model.in_channels if model.roll_out else model.in_channels
+    zs = torch.randn(num_samples, C, model.input_size, model.input_size).to(dev).to(dtype).float()
+    ctx = {}
+    for k in c:
+        if k in ("vector", "crossattn", "concat"):
+            ctx[k] = torch.cat((c[k], uc[k]), 0).to(dev).to(dtype).float().contiguous()
+        else:
+            assert c[k] == uc[k]
+            ctx[k] = c[k]
+    fn = Sampler(create_transport(snr_type="lognorm")).sample_ode(sampling_method=sampling_method, num_steps=num_steps)
+    samples = fn(torch.cat([zs, zs], 0), model.forward_with_cfg, context=ctx, cfg_scale=cfg_scale)[-1]
+    return samples.chunk(2, dim=0)[0]
+
+
+@torch.no_grad()
+def _cond_to_3d(conditioner, model, decoder, cond_key, prompt, cameras, num_samples, seed, num_steps, cfg_scale,
+                sampling_method, resolution, dtype):
+    dev = next(model.parameters()).device
+    c, uc = condition_prompt(conditioner, cond_key, prompt, num_samples, device=dev)
+    latents = sample_flow(model, c, uc, num_samples, seed=seed, num_steps=num_steps, cfg_scale=cfg_scale,
+                          sampling_method=sampling_method, dtype=dtype)
+    return latents, decode_and_render(decoder, latents, cameras[:24].to(dev), resolution)
+
+
+@torch.no_grad()
+def mv_to_3d(conditioner, model, decoder, mv_images: torch.Tensor, mv_cameras: torch.Tensor, cameras: torch.Tensor,
+             num_samples: int = 4, seed: int = 42, num_steps: int = 250, cfg_scale: float = 4.0,
+             sampling_method: str = "dopri5", resolution: int = 192, dtype=torch.float32):
+    """Multi-view-to-3D, `FlowMatchingEngine.eval_cldm` for cond_key 'img-c' (nsr/lsgm/flow_matching_trainer.py:
+    553-678): the conditioner on {'img': mv_images (1, V, 3, H, W) in [-1, 1], 'c': mv_cameras (1, V, 25)} with the
+    unconditional half forced to zero and every row repeated `num_samples` times, `sample_flow`, then decode and render
+    of `cameras[:24]` at `resolution`.  The release (sample_obajverse_mv23d_dit.sh) runs 6 views, 4 samples, CFG 4.0,
+    dopri5 with 250 output points and 192^2 renders.
+
+    The engine casts the views and cameras to its dtype (bf16 under use_amp) before the conditioner sees them; they
+    are cast to `dtype` here.  With `aug_c=True` the conditioner rotates cameras of that tensor in place -- the caller's
+    own `mv_cameras` when it already has that dtype and device.  Returns (latents, render dict)."""
+    dev = next(model.parameters()).device
+    img_c = {"img": mv_images.to(dev).to(dtype), "c": mv_cameras.to(dev).to(dtype)}
+    return _cond_to_3d(conditioner, model, decoder, "img-c", img_c, cameras, num_samples, seed, num_steps, cfg_scale,
+                       sampling_method, resolution, dtype)
+
+
+@torch.no_grad()
+def image_to_3d(conditioner, model, decoder, image: torch.Tensor, cameras: torch.Tensor, num_samples: int = 4,
+                seed: int = 42, num_steps: int = 250, cfg_scale: float = 4.0, sampling_method: str = "dopri5",
+                resolution: int = 192, dtype=torch.float32):
+    """Image-to-3D, `FlowMatchingEngine.eval_cldm` for cond_key 'img' (the I23D release): the conditioner on one image
+    (1, 3, H, W) in [-1, 1], `sample_flow`, decode and render of `cameras[:24]`.  Returns (latents, render dict)."""
+    dev = next(model.parameters()).device
+    return _cond_to_3d(conditioner, model, decoder, "img", image.to(dev).to(dtype), cameras, num_samples, seed,
+                       num_steps, cfg_scale, sampling_method, resolution, dtype)
+
+
 # ---------------------------------------------------------------------------------------------- multi-GPU
 def shard_range(n_total: int, world: int, rank: int) -> tuple[int, int, int]:
     """Contiguous block of ceil(P/G) prompts per rank (SURVEY.md section 8e): returns (lo, hi, per) with

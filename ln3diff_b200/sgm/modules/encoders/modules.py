@@ -1,8 +1,8 @@
 """Mirror of the conditioner stack of reference sgm/modules/encoders/modules.py (SURVEY 8f-1):
-`GeneralConditioner` (:80-190), `FrozenCLIPEmbedder` (:347-408, T23D), `FrozenOpenCLIPImageEmbedder` (:578-733)
-and `FrozenDinov2ImageEmbedder` (:735-868, I23D) -- same class names, constructor arguments, `input_key` /
-`ucg_rate` plumbing, output shapes and dictionary keys; the three frozen towers run on the libln3b200 kernels
-(`_tower.TransformerTower`) instead of transformers / open_clip / the dinov2 hub model.
+`GeneralConditioner` (:80-190), `FrozenCLIPEmbedder` (:347-408, T23D), `FrozenOpenCLIPImageEmbedder` (:578-733),
+`FrozenDinov2ImageEmbedder` (:735-868, I23D) and `FrozenDinov2ImageEmbedderMVPlucker` (:871-1104, MV23D) -- same class
+names, constructor arguments, `input_key` / `ucg_rate` plumbing, output shapes and dictionary keys; the frozen towers
+run on the libln3b200 kernels (`_tower.TransformerTower`) instead of transformers / open_clip / the dinov2 hub model.
 
 Weights.  The reference constructors download pretrained weights (`CLIPTextModel.from_pretrained`,
 `open_clip.create_model_and_transforms`, `torch.hub.load`).  There is no network here: every embedder takes
@@ -27,6 +27,7 @@ Third-party arithmetic restated here (file:line = reference call site):
 from __future__ import annotations
 
 import math
+import random
 from contextlib import nullcontext
 from typing import Dict, List, Optional, Union
 
@@ -502,21 +503,7 @@ class FrozenDinov2ImageEmbedder(_ImageEmbedderBase):
                 return {"model." + k: v for k, v in model.state_dict().items()}
             state_dict = _load_pretrained("FrozenDinov2ImageEmbedder", _load)
         if state_dict is None:
-            g = torch.Generator().manual_seed(seed)
-            sd = {"cls_token": _randn(1, 1, width, g=g), "register_tokens": _randn(1, num_register_tokens, width, g=g),
-                  "pos_embed": _randn(1, 1 + pos_grid * pos_grid, width, g=g),
-                  "patch_embed.proj.weight": _randn(width, 3, patch, patch, g=g), "patch_embed.proj.bias": _randn(width, g=g),
-                  "norm.weight": torch.ones(width), "norm.bias": torch.zeros(width)}
-            for i in range(depth):
-                p = f"blocks.{i}."
-                sd[p + "attn.qkv.weight"], sd[p + "attn.qkv.bias"] = _randn(3 * width, width, g=g), _randn(3 * width, g=g)
-                sd[p + "attn.proj.weight"], sd[p + "attn.proj.bias"] = _randn(width, width, g=g), _randn(width, g=g)
-                sd[p + "mlp.fc1.weight"], sd[p + "mlp.fc1.bias"] = _randn(mlp_dim, width, g=g), _randn(mlp_dim, g=g)
-                sd[p + "mlp.fc2.weight"], sd[p + "mlp.fc2.bias"] = _randn(width, mlp_dim, g=g), _randn(width, g=g)
-                sd[p + "ls1.gamma"], sd[p + "ls2.gamma"] = torch.full((width,), 0.5), torch.full((width,), 0.5)
-                for ln in ("norm1", "norm2"):
-                    sd[p + ln + ".weight"], sd[p + ln + ".bias"] = torch.ones(width), torch.zeros(width)
-            state_dict = sd
+            state_dict = self._random_state_dict(width, depth, mlp_dim, patch, num_register_tokens, pos_grid, seed)
         sd = _strip(state_dict, "model.")
         dev = torch.device(device)
         width = sd["cls_token"].shape[-1]
@@ -540,6 +527,25 @@ class FrozenDinov2ImageEmbedder(_ImageEmbedderBase):
         self._norm = _ln_pair(sd["norm.weight"], sd["norm.bias"], dev)
         if freeze:
             self.freeze()
+
+    @staticmethod
+    def _random_state_dict(width, depth, mlp_dim, patch, num_register_tokens, pos_grid, seed, in_chans=3) -> dict:
+        """random_init=True: a seeded DINOv2-with-registers state dict (hub key layout, no `model.` prefix)."""
+        g = torch.Generator().manual_seed(seed)
+        sd = {"cls_token": _randn(1, 1, width, g=g), "register_tokens": _randn(1, num_register_tokens, width, g=g),
+              "pos_embed": _randn(1, 1 + pos_grid * pos_grid, width, g=g),
+              "patch_embed.proj.weight": _randn(width, in_chans, patch, patch, g=g), "patch_embed.proj.bias": _randn(width, g=g),
+              "norm.weight": torch.ones(width), "norm.bias": torch.zeros(width)}
+        for i in range(depth):
+            p = f"blocks.{i}."
+            sd[p + "attn.qkv.weight"], sd[p + "attn.qkv.bias"] = _randn(3 * width, width, g=g), _randn(3 * width, g=g)
+            sd[p + "attn.proj.weight"], sd[p + "attn.proj.bias"] = _randn(width, width, g=g), _randn(width, g=g)
+            sd[p + "mlp.fc1.weight"], sd[p + "mlp.fc1.bias"] = _randn(mlp_dim, width, g=g), _randn(mlp_dim, g=g)
+            sd[p + "mlp.fc2.weight"], sd[p + "mlp.fc2.bias"] = _randn(width, mlp_dim, g=g), _randn(width, g=g)
+            sd[p + "ls1.gamma"], sd[p + "ls2.gamma"] = torch.full((width,), 0.5), torch.full((width,), 0.5)
+            for ln in ("norm1", "norm2"):
+                sd[p + ln + ".weight"], sd[p + ln + ".bias"] = torch.ones(width), torch.zeros(width)
+        return sd
 
     def interpolate_pos_encoding(self, n_side: int) -> torch.Tensor:
         """dinov2 DinoVisionTransformer.interpolate_pos_encoding for an n_side x n_side patch grid."""
@@ -567,11 +573,12 @@ class FrozenDinov2ImageEmbedder(_ImageEmbedderBase):
         return out
 
     @torch.no_grad()
-    def forward_features(self, img: torch.Tensor) -> dict:
-        """dinov2 forward_features on a pre-processed batch (B,3,H,W), H = W = 14 n."""
+    def forward_features(self, img: torch.Tensor, patch_tokens: Optional[torch.Tensor] = None) -> dict:
+        """dinov2 forward_features on a pre-processed batch (B,3,H,W), H = W = 14 n.  `patch_tokens` (B, n*n, D):
+        the patch embedding already computed by the caller (the 9-channel input of the multi-view embedder)."""
         B = img.shape[0]
         n = img.shape[-1] // self.patch
-        x = _patchify_gemm(img, self._conv_w, self._conv_b, self.patch)
+        x = _patchify_gemm(img, self._conv_w, self._conv_b, self.patch) if patch_tokens is None else patch_tokens
         x = torch.cat([self.cls_token.expand(B, -1, -1), x], dim=1) + self.interpolate_pos_encoding(n)
         R = self.register_tokens.shape[1]
         x = torch.cat([x[:, :1], self.register_tokens.expand(B, -1, -1), x[:, 1:]], dim=1).contiguous()
@@ -604,3 +611,114 @@ class FrozenDinov2ImageEmbedder(_ImageEmbedderBase):
         if self.output_cls:
             return tokens, z
         return tokens
+
+
+# --------------------------------------------------------------------------------------------- multi-view DINOv2
+def _nine_channel_patch_embed(state_dict: dict) -> dict:
+    """The reference constructor's patch-embedding surgery (:922-938): a 3-channel `patch_embed.proj.weight` becomes a
+    zero-initialised 9-channel one whose first three input channels are the pretrained weights (the bias is kept).
+    A state dict that already holds the 9-channel weight (a trained MV23D checkpoint) is returned unchanged."""
+    sd = dict(state_dict)
+    for k in ("model.patch_embed.proj.weight", "patch_embed.proj.weight"):
+        w = sd.get(k)
+        if w is not None and w.shape[1] == 3:
+            w9 = torch.zeros(w.shape[0], 9, *w.shape[2:], dtype=w.dtype)
+            w9[:, :3] = w.detach().cpu()
+            sd[k] = w9
+    return sd
+
+
+class FrozenDinov2ImageEmbedderMVPlucker(FrozenDinov2ImageEmbedder):
+    """The multi-view conditioner of the MV23D release (reference :871-1104; config
+    sgm/configs/mv23d-plucker-clipl-compat-fm-lognorm-noclip.yaml: arch='vitb', enable_bf16=True, n_cond_frames=6,
+    modLN=False, aug_c=True, input_key 'img-c'): DINOv2 ViT-B/14 with 4 registers whose patch embedding takes 9
+    channels, RGB plus the Plücker ray [o x d, d] of every pixel of the 224 x 224 view.  forward({'img': (B,V,3,H,W),
+    'c': (B,V,25)}) -> normalised patch tokens (B, n_cond_frames, 256, width), which GeneralConditioner files under
+    'concat'.
+
+    The 9-channel patch operand comes from one kernel (ops.plucker_patchify: rays, cat, bf16 cast and im2col) and the
+    patch embedding from one GEMM; the tower is FrozenDinov2ImageEmbedder's.  The operand is bf16 whatever
+    `enable_bf16` says: under the engine's bf16 autocast the reference's patch-embedding conv rounds it to bf16 too.
+    `modLN` is accepted and ignored, as in the reference.
+
+    aug_c=True rotates each conditioning camera with probability 0.4 before the rays are built -- at inference too,
+    as the reference does (:1079-1088): `random.random()` per (b, v) and, on a hit, `np.random.uniform` for the angle
+    and `random.random()` for the axis, rotating the caller's camera tensor in place, in its dtype."""
+
+    def __init__(self, arch="vitl", version="dinov2", device="cuda", max_length=77, freeze=True, antialias=True,
+                 ucg_rate=0.0, unsqueeze_dim=False, repeat_to_max_len=False, num_image_crops=0, output_tokens=False,
+                 output_cls=False, init_device=None, n_cond_frames=4, enable_bf16=False, modLN=False, aug_c=False, *,
+                 state_dict: dict | None = None, random_init: bool = False, width=768, depth=12, mlp_dim=3072, patch=14,
+                 num_register_tokens=4, pos_grid=37, interpolate_antialias=True, interpolate_offset=0.0, seed=0):
+        if output_cls:
+            raise NotImplementedError("FrozenDinov2ImageEmbedderMVPlucker: output_cls (the reference cannot run it either)")
+        if state_dict is None and not random_init:
+            def _load():
+                model = torch.hub.load(f"facebookresearch/{version}", f"{version}_{arch}14_reg", pretrained=True)  # :760-765
+                return {"model." + k: v for k, v in model.state_dict().items()}
+            state_dict = _load_pretrained("FrozenDinov2ImageEmbedderMVPlucker", _load)
+        if state_dict is None:
+            state_dict = FrozenDinov2ImageEmbedder._random_state_dict(width, depth, mlp_dim, patch, num_register_tokens,
+                                                                      pos_grid, seed, in_chans=9)
+        super().__init__(arch, version, device, max_length, freeze, antialias, ucg_rate, unsqueeze_dim, repeat_to_max_len,
+                         num_image_crops, output_tokens, output_cls, init_device,
+                         state_dict=_nine_channel_patch_embed(state_dict), interpolate_antialias=interpolate_antialias,
+                         interpolate_offset=interpolate_offset)
+        if self.patch != 14 or self._conv_w.shape[1] != 1792:
+            raise NotImplementedError("FrozenDinov2ImageEmbedderMVPlucker: a 9-channel 14x14 patch embedding is required")
+        self.n_cond_frames = n_cond_frames
+        self.enable_bf16 = enable_bf16
+        self.dtype = torch.bfloat16 if enable_bf16 else torch.float32
+        self.aug_c = aug_c
+        self.reso_encoder = 224
+
+    def preprocess(self, x):
+        """reference :1015-1047.  Its ucg_rate > 0 branch (scale jitter and Gaussian noise) runs only outside
+        get_unconditional_conditioning, i.e. in training."""
+        if self.ucg_rate > 0.0:
+            raise NotImplementedError("FrozenDinov2ImageEmbedderMVPlucker with ucg_rate > 0: the reference's "
+                                      "training-time augmentation is not implemented (inference runs through "
+                                      "GeneralConditioner.get_unconditional_conditioning, which sets ucg_rate = 0)")
+        return super().preprocess(x)
+
+    @staticmethod
+    def random_rotate_c(c: torch.Tensor) -> torch.Tensor:
+        """reference :1049-1076: a random rotation about z or y (InstantMesh's camera augmentation) applied to the
+        cam2world of one (25,) camera row, in the row's dtype.  RNG: np.random.uniform, then random.random()."""
+        intrinsics, c2ws = c[16:], c[:16].reshape(4, 4)
+        degree = np.random.uniform(0, math.pi * 2)
+        cs, sn = np.cos(degree), np.sin(degree)
+        if random.random() > 0.5:
+            rot = [[cs, -sn, 0, 0], [sn, cs, 0, 0], [0, 0, 1, 0], [0, 0, 0, 1]]
+        else:
+            rot = [[cs, 0, sn, 0], [0, 1, 0, 0], [-sn, 0, cs, 0], [0, 0, 0, 1]]
+        rot = torch.tensor(rot).to(c2ws)
+        return torch.cat([torch.matmul(rot, c2ws).reshape(-1), intrinsics])
+
+    @classmethod
+    def augment_cameras(cls, c: torch.Tensor) -> torch.Tensor:
+        """aug_c (reference :1084-1088): every camera of c (B, V, 25) is rotated, in place, with probability 0.4."""
+        for b in range(c.shape[0]):
+            for v in range(c.shape[1]):
+                if random.random() > 0.6:
+                    c[b, v] = cls.random_rotate_c(c[b, v])
+        return c
+
+    def encode_with_vision_transformer(self, img, cams=None, **kwargs):
+        """(B*V, 3, H, W) views + (B*V, 25) cameras -> patch tokens (B*V, 256, width)."""
+        if img.dim() == 5:
+            img = img.reshape(-1, *img.shape[2:])
+        dev = self.cls_token.device
+        img = self.preprocess(img.to(dev)).contiguous()
+        a = ops.plucker_patchify(img, cams.to(device=dev, dtype=torch.float32).contiguous(), ldo=self._conv_w.shape[1])
+        patches = ops.gemm(a, self._conv_w, self._conv_b).float().view(img.shape[0], -1, self._conv_w.shape[0])
+        return self.forward_features(img, patch_tokens=patches)["x_norm_patchtokens"]
+
+    def forward(self, img_c, no_dropout=False):
+        mv_image, c = img_c["img"], img_c["c"]
+        if self.aug_c:
+            self.augment_cameras(c)
+        B, V = mv_image.shape[0], self.n_cond_frames
+        cams = c[:, :V].reshape(-1, c.shape[-1])
+        tokens = super().forward(mv_image[:, :V], no_dropout=no_dropout, cams=cams)
+        return tokens.reshape(B, -1, *tokens.shape[1:])

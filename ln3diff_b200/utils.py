@@ -63,6 +63,23 @@ def build_i23d(arch: str = "DiT-PixArt-L/2", seed: int = 0, device: str | None =
     return m.to(device) if device else m
 
 
+def build_mv23d(arch: str = "DiT-PixArt-MV-L/2", seed: int = 0, device: str | None = None, **kwargs):
+    """Multi-view denoiser as the MV23D release builds it (DiT_models_i23d['DiT-PixArt-MV-L/2'](...,
+    context_dim=768, pooling_ctx_dim=768, learn_sigma=False), guided_diffusion/script_util.py:397-406);
+    `kwargs` override the registry sizes (depth, hidden_size, num_heads) for reduced test models."""
+    from .dit.dit_i23d import DiT_I23D_PixelArt_MVCond_noClip, DiT_models
+    torch.manual_seed(seed)
+    args = dict(input_size=32, num_classes=0, learn_sigma=False, in_channels=4, context_dim=768, pooling_ctx_dim=768,
+                roll_out=True)
+    if kwargs:
+        m = DiT_I23D_PixelArt_MVCond_noClip(patch_size=2, **{**args, **kwargs})
+    else:
+        m = DiT_models[arch](**args)
+    derandomize_zero_init(m)
+    m.eval()
+    return m.to(device) if device else m
+
+
 def orbit_cameras(V: int, radius: float = 1.7, focal: float = 1.3889) -> torch.Tensor:
     """(V, 25) synthetic camera rows in the layout of the reference's assets/objv_eval_pose.pt:
     16 row-major cam2world (OpenCV convention, looking at the origin) + 9 normalised intrinsics
