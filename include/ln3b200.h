@@ -473,6 +473,42 @@ int ln3_attn_single_head(const float* q, const float* k, const float* v, float* 
 int ln3_patch_embed_triplane(const float* x, const float* w, const float* bias, int B, int Cz, int S,
                              int E, float in_mul, float* tokens, void* silu_bf16, void* stream);
 
+/* ------------------------------------------------------------------ VAE encoder (NHWC fp32)
+ * The stage-1 encoder MVEncoder (ldm/modules/diffusionmodules/model.py:459-577) runs on ln3_conv_nhwc,
+ * ln3_groupnorm_stats, ln3_gemm_bf16, ln3_fmha_fwd and ln3_norm_modulate plus the two entry points below.
+ *
+ * ln3_downsample_nhwc: Downsample (model.py:72-91): out = conv3x3(F.pad(x, (0,1,0,1)), stride 2, no padding) + bias.
+ *   Here H, W are the INPUT dims and must be even; x [N, H, W, Cin], out [N, H/2, W/2, Cout], w repacked to
+ *   [9, Cin, Cout] as for ln3_conv_nhwc.  precision LN3_MLP_FP32 (exact SIMT) or LN3_MLP_TF32 (mma.sync, fp32
+ *   accumulate).  LN3_EINVAL for odd H or W, ksize != 3, upsample, in_scale / in_shift, residual, another precision,
+ *   non-positive sizes or a NULL x, w or out.
+ *
+ * ln3_vae_posterior: vae_encode + DiagonalGaussianDistribution(soft_clamp=True) + sample() / mode() of the AE
+ *   decoder (vit/vit_triplane.py:912-933, 1152-1199; utils/torch_utils/distributions/distributions.py:29-113):
+ *     moments fp32 [B, S, S, 24]  the fused encoder output, NHWC
+ *     w fp32 [24, 8], bias [24]   quant_conv = Conv2d(24, 24, 1, groups=3)
+ *     noise fp32 [B, 12, S, S]    the standard-normal draw of sample(), or NULL for mode(): z = mean
+ *     mean, logvar, z fp32 [B, 12, S, S] (the layout of latent_normalized_2Ddiffusion)
+ *   with q = quant_conv(moments), mean[:, j] = q[:, j], lv = q[:, 12 + j] (the reference's reshape to (B, 8, 3, H, W)
+ *   and chunk), logvar = 20 tanh(lv / 20), z = mean + exp(0.5 logvar) * noise.  Each fp32 step after the 8-term dot
+ *   product is rounded on its own, as torch evaluates it.  LN3_EINVAL for B < 0, S <= 0 or a NULL pointer other than
+ *   noise.
+ */
+int ln3_downsample_nhwc(const ln3_conv_args* args, void* stream);
+
+typedef struct ln3_vae_posterior_args {
+  const float* moments;
+  const float* w;
+  const float* bias;
+  const float* noise;
+  float* mean;
+  float* logvar;
+  float* z;
+  int B, S;
+} ln3_vae_posterior_args;
+
+int ln3_vae_posterior(const ln3_vae_posterior_args* args, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -152,6 +152,14 @@ class ConvArgs(C.Structure):
     ]
 
 
+class VaePosteriorArgs(C.Structure):
+    _fields_ = [
+        ("moments", C.c_void_p), ("w", C.c_void_p), ("bias", C.c_void_p), ("noise", C.c_void_p),
+        ("mean", C.c_void_p), ("logvar", C.c_void_p), ("z", C.c_void_p),
+        ("B", C.c_int), ("S", C.c_int),
+    ]
+
+
 NORM_NONE, NORM_LAYER, NORM_RMS = 0, 1, 2
 MLP_FP32, MLP_TF32 = 0, 1
 

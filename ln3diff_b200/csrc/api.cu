@@ -202,4 +202,13 @@ int ln3_patch_embed_triplane(const float* x, const float* w, const float* bias, 
                               static_cast<cudaStream_t>(stream));
 }
 
+int ln3_downsample_nhwc(const ln3_conv_args* args, void* stream) {
+  if (!args) return set_error(LN3_EINVAL, "downsample: null args");
+  return downsample_nhwc(args, static_cast<cudaStream_t>(stream));
+}
+int ln3_vae_posterior(const ln3_vae_posterior_args* args, void* stream) {
+  if (!args) return set_error(LN3_EINVAL, "vae_posterior: null args");
+  return vae_posterior(args, static_cast<cudaStream_t>(stream));
+}
+
 }  // extern "C"

@@ -28,20 +28,33 @@ namespace ln3 {
 // Block: 8x8 output pixels x COT output channels; 256 threads = 64 pixels x 4 channel groups, each
 // thread accumulates COT/4 channels.  Input channels are consumed in chunks of 16 staged in smem as
 // [cin][10x10 halo tile] (pixel fastest -> conflict-free reads), weights as [tap][cin][COT].
+//
+// DOWN = the encoder's Downsample (ldm/modules/diffusionmodules/model.py:72-91): F.pad(x, (0,1,0,1)) then a 3x3
+// conv with stride 2 and no padding.  a.H, a.W are then the (even) INPUT dims; the 8x8 output tile reads input rows
+// and columns [2*t0, 2*t0 + 17), a 17x17 tile whose last row / column is the zero pad at the image edge.  Each
+// staged row is stored de-interleaved -- even columns at positions 0..8, odd columns at 9..16 -- so that the eight
+// output columns of one tap read eight consecutive words.
 static constexpr int kCT = 8;        // tile edge (pixels)
 static constexpr int kCinChunk = 16;
+static constexpr int kDownTW = 2 * kCT + 1;   // staged tile edge of the stride-2 conv
 
-template <int COT, int KS>
+// staged position of tile column c (0..16) in a de-interleaved stride-2 row, and its inverse
+__device__ __forceinline__ int down_pos(int c) { return (c & 1) ? 9 + (c >> 1) : (c >> 1); }
+__device__ __forceinline__ int down_col(int p) { return p < 9 ? 2 * p : 2 * (p - 9) + 1; }
+
+template <int COT, int KS, bool DOWN>
 __global__ void __launch_bounds__(256)
 conv_nhwc_kernel(const ln3_conv_args a) {
-  constexpr int HALO = (KS == 3) ? 1 : 0;
-  constexpr int TW = kCT + 2 * HALO;           // staged tile edge
+  static_assert(!DOWN || KS == 3, "the stride-2 conv is 3x3");
+  constexpr int HALO = (KS == 3 && !DOWN) ? 1 : 0;
+  constexpr int TW = DOWN ? kDownTW : kCT + 2 * HALO;   // staged tile edge
   constexpr int NACC = COT / 4;
   __shared__ float s_in[kCinChunk][TW * TW + 1];
   __shared__ __align__(16) float s_w[KS * KS][kCinChunk][COT];
 
   const int n = blockIdx.z;
-  const int tiles_x = (a.W + kCT - 1) / kCT;
+  const int Ho = DOWN ? a.H / 2 : a.H, Wo = DOWN ? a.W / 2 : a.W;
+  const int tiles_x = (Wo + kCT - 1) / kCT;
   const int ty0 = (blockIdx.x / tiles_x) * kCT, tx0 = (blockIdx.x % tiles_x) * kCT;
   const int co0 = blockIdx.y * COT;
   const int pix = threadIdx.x & 63, q = threadIdx.x >> 6;
@@ -56,7 +69,8 @@ conv_nhwc_kernel(const ln3_conv_args a) {
     // stage input tile (GroupNorm-apply + swish + nearest upsample fused into the load)
     for (int i = threadIdx.x; i < TW * TW * kCinChunk; i += 256) {
       const int ci = i % kCinChunk, t = i / kCinChunk;   // channel fastest in gmem (NHWC)
-      const int yy = ty0 + t / TW - HALO, xx = tx0 + t % TW - HALO;
+      const int yy = DOWN ? 2 * ty0 + t / TW : ty0 + t / TW - HALO;
+      const int xx = DOWN ? 2 * tx0 + down_col(t % TW) : tx0 + t % TW - HALO;
       float v = 0.f;
       if (yy >= 0 && yy < a.H && xx >= 0 && xx < a.W && c0 + ci < a.Cin) {
         const int ys = a.upsample ? (yy >> 1) : yy, xs = a.upsample ? (xx >> 1) : xx;
@@ -79,7 +93,7 @@ conv_nhwc_kernel(const ln3_conv_args a) {
     __syncthreads();
 #pragma unroll
     for (int tap = 0; tap < KS * KS; ++tap) {
-      const int t = (py + tap / KS) * TW + (px + tap % KS);
+      const int t = DOWN ? (2 * py + tap / 3) * TW + down_pos(2 * px + tap % 3) : (py + tap / KS) * TW + (px + tap % KS);
 #pragma unroll 4
       for (int ci = 0; ci < kCinChunk; ++ci) {
         const float xv = s_in[ci][t];
@@ -97,8 +111,8 @@ conv_nhwc_kernel(const ln3_conv_args a) {
     __syncthreads();
   }
   const int oy = ty0 + py, ox = tx0 + px;
-  if (oy < a.H && ox < a.W) {
-    const long long o = ((static_cast<long long>(n) * a.H + oy) * a.W + ox) * a.Cout + co0 + q * NACC;
+  if (oy < Ho && ox < Wo) {
+    const long long o = ((static_cast<long long>(n) * Ho + oy) * Wo + ox) * a.Cout + co0 + q * NACC;
 #pragma unroll
     for (int i = 0; i < NACC; ++i) {
       const int co = co0 + q * NACC + i;
@@ -117,19 +131,21 @@ conv_nhwc_kernel(const ln3_conv_args a) {
 // issued as mma.sync.m16n8k8 TF32 (fp32 accumulate): 72 MMAs + 216 LDS per warp and chunk instead of
 // 2304 FFMA + 720 LDS per thread.  Warp w: pixel rows 2*(w&3), 2*(w&3)+1 of the 8x8 tile (one m-tile),
 // channel half w>>2.  smem rows are padded to strides = 8 (mod 32) words so that the (g, t) fragment
-// pattern of a warp touches 32 distinct banks.
-template <int COT>
+// pattern of a warp touches 32 distinct banks.  DOWN: the stride-2 Downsample conv on the 17x17 de-interleaved tile of
+// conv_nhwc_kernel (a.H, a.W = input dims); the eight A rows g of one tap are then eight consecutive staged words.
+template <int COT, bool DOWN>
 __global__ void __launch_bounds__(256)
 conv3x3_tf32_kernel(const ln3_conv_args a) {
-  constexpr int TW = kCT + 2;            // staged tile edge (halo 1)
-  constexpr int SIN = 104;               // >= TW*TW, = 8 (mod 32)
+  constexpr int TW = DOWN ? kDownTW : kCT + 2;   // staged tile edge
+  constexpr int SIN = DOWN ? 296 : 104;          // >= TW*TW, = 8 (mod 32)
   constexpr int SW = COT + 8;            // = 8 (mod 32)
   constexpr int NT = COT / 16;           // n-tiles (of 8 channels) per warp
   __shared__ uint32_t s_in[kCinChunk][SIN];
   __shared__ uint32_t s_w[9][kCinChunk][SW];
 
   const int n = blockIdx.z;
-  const int tiles_x = (a.W + kCT - 1) / kCT;
+  const int Ho = DOWN ? a.H / 2 : a.H, Wo = DOWN ? a.W / 2 : a.W;
+  const int tiles_x = (Wo + kCT - 1) / kCT;
   const int ty0 = (blockIdx.x / tiles_x) * kCT, tx0 = (blockIdx.x % tiles_x) * kCT;
   const int co0 = blockIdx.y * COT;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -144,7 +160,8 @@ conv3x3_tf32_kernel(const ln3_conv_args a) {
   for (int c0 = 0; c0 < a.Cin; c0 += kCinChunk) {
     for (int i = threadIdx.x; i < TW * TW * kCinChunk; i += 256) {
       const int ci = i % kCinChunk, tt = i / kCinChunk;   // channel fastest in gmem (NHWC)
-      const int yy = ty0 + tt / TW - 1, xx = tx0 + tt % TW - 1;
+      const int yy = DOWN ? 2 * ty0 + tt / TW : ty0 + tt / TW - 1;
+      const int xx = DOWN ? 2 * tx0 + down_col(tt % TW) : tx0 + tt % TW - 1;
       float v = 0.f;
       if (yy >= 0 && yy < a.H && xx >= 0 && xx < a.W && c0 + ci < a.Cin) {
         const int ys = a.upsample ? (yy >> 1) : yy, xs = a.upsample ? (xx >> 1) : xx;
@@ -167,11 +184,12 @@ conv3x3_tf32_kernel(const ln3_conv_args a) {
 #pragma unroll
     for (int tap = 0; tap < 9; ++tap) {
       // A rows: g -> pixel (2*mt, g), g + 8 -> pixel (2*mt + 1, g); shifted by the tap inside the halo tile
-      const int p0 = (2 * mt + tap / 3) * TW + g + tap % 3;
+      const int p0 = DOWN ? (4 * mt + tap / 3) * TW + down_pos(2 * g + tap % 3) : (2 * mt + tap / 3) * TW + g + tap % 3;
+      constexpr int DR = DOWN ? 2 * TW : TW;   // staged distance between the two output rows
 #pragma unroll
       for (int ks = 0; ks < 2; ++ks) {
-        const uint32_t af[4] = {s_in[8 * ks + t][p0], s_in[8 * ks + t][p0 + TW], s_in[8 * ks + t + 4][p0],
-                                s_in[8 * ks + t + 4][p0 + TW]};
+        const uint32_t af[4] = {s_in[8 * ks + t][p0], s_in[8 * ks + t][p0 + DR], s_in[8 * ks + t + 4][p0],
+                                s_in[8 * ks + t + 4][p0 + DR]};
 #pragma unroll
         for (int nt = 0; nt < NT; ++nt) {
           const int cb = nh * (COT / 2) + nt * 8 + g;
@@ -185,8 +203,8 @@ conv3x3_tf32_kernel(const ln3_conv_args a) {
 #pragma unroll
   for (int half = 0; half < 2; ++half) {
     const int oy = ty0 + 2 * mt + half, ox = tx0 + g;
-    if (oy < a.H && ox < a.W) {
-      const long long o = ((static_cast<long long>(n) * a.H + oy) * a.W + ox) * a.Cout;
+    if (oy < Ho && ox < Wo) {
+      const long long o = ((static_cast<long long>(n) * Ho + oy) * Wo + ox) * a.Cout;
 #pragma unroll
       for (int nt = 0; nt < NT; ++nt) {
         const int co = co0 + nh * (COT / 2) + nt * 8 + 2 * t;
@@ -218,17 +236,97 @@ int conv_nhwc(const ln3_conv_args* a, cudaStream_t stream) {
   if (cot == 64 && cot_auto && static_cast<long long>(tiles) * ((a->Cout + 63) / 64) * a->N < 2 * device_sm_count()) cot = 32;
   dim3 grid(tiles, (a->Cout + cot - 1) / cot, a->N);
   if (a->ksize == 3 && a->precision == LN3_MLP_TF32) {
-    if (cot == 64) conv3x3_tf32_kernel<64><<<grid, 256, 0, stream>>>(*a);
-    else conv3x3_tf32_kernel<32><<<grid, 256, 0, stream>>>(*a);
+    if (cot == 64) conv3x3_tf32_kernel<64, false><<<grid, 256, 0, stream>>>(*a);
+    else conv3x3_tf32_kernel<32, false><<<grid, 256, 0, stream>>>(*a);
   } else if (a->ksize == 3) {
-    if (cot == 64) conv_nhwc_kernel<64, 3><<<grid, 256, 0, stream>>>(*a);
-    else conv_nhwc_kernel<32, 3><<<grid, 256, 0, stream>>>(*a);
+    if (cot == 64) conv_nhwc_kernel<64, 3, false><<<grid, 256, 0, stream>>>(*a);
+    else conv_nhwc_kernel<32, 3, false><<<grid, 256, 0, stream>>>(*a);
   } else {
-    if (cot == 64) conv_nhwc_kernel<64, 1><<<grid, 256, 0, stream>>>(*a);
-    else conv_nhwc_kernel<32, 1><<<grid, 256, 0, stream>>>(*a);
+    if (cot == 64) conv_nhwc_kernel<64, 1, false><<<grid, 256, 0, stream>>>(*a);
+    else conv_nhwc_kernel<32, 1, false><<<grid, 256, 0, stream>>>(*a);
   }
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error(LN3_ECUDA, "conv launch: %s", cudaGetErrorString(e));
+  count_launch();
+  return LN3_OK;
+}
+
+// 32 output channels per CTA: the 17x17 staged tile with 64 channels of weights would exceed 48 KB of static smem
+// (TF32: 18.9 KB input + 41.5 KB weights).  The encoder's three Downsample convs have 64..256 channels, so the grid
+// is tiles x Cout/32 x views: 2048 / 1024 / 512 CTAs per 4 views.
+int downsample_nhwc(const ln3_conv_args* a, cudaStream_t stream) {
+  if (a->ksize != 3) return set_error(LN3_EINVAL, "downsample: ksize must be 3");
+  if (a->upsample) return set_error(LN3_EINVAL, "downsample: upsample is not supported");
+  if (a->in_scale != nullptr || a->in_shift != nullptr)
+    return set_error(LN3_EINVAL, "downsample: in_scale / in_shift (fused GroupNorm) are not supported");
+  if (a->residual != nullptr) return set_error(LN3_EINVAL, "downsample: residual is not supported");
+  if (a->precision != LN3_MLP_FP32 && a->precision != LN3_MLP_TF32)
+    return set_error(LN3_EINVAL, "downsample: precision must be LN3_MLP_FP32 or LN3_MLP_TF32");
+  if (a->N < 0 || a->H <= 0 || a->W <= 0 || a->Cin <= 0 || a->Cout <= 0)
+    return set_error(LN3_EINVAL, "downsample: need N >= 0 and positive H, W, Cin, Cout");
+  if ((a->H | a->W) & 1) return set_error(LN3_EINVAL, "downsample: H, W (input dims) must be even");
+  if (!a->x || !a->w || !a->out) return set_error(LN3_EINVAL, "downsample: null pointer");
+  if (a->N == 0) return LN3_OK;
+  const int tiles = ((a->H / 2 + kCT - 1) / kCT) * ((a->W / 2 + kCT - 1) / kCT);
+  dim3 grid(tiles, (a->Cout + 31) / 32, a->N);
+  if (a->precision == LN3_MLP_TF32) conv3x3_tf32_kernel<32, true><<<grid, 256, 0, stream>>>(*a);
+  else conv_nhwc_kernel<32, 3, true><<<grid, 256, 0, stream>>>(*a);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return set_error(LN3_ECUDA, "downsample launch: %s", cudaGetErrorString(e));
+  count_launch();
+  return LN3_OK;
+}
+
+// ------------------------------------------------------------------ VAE posterior (quant_conv + DiagonalGaussian)
+// One thread per (object, pixel): the 24 fused moments of the pixel (NHWC) -> grouped 1x1 quant_conv (out channel o
+// reads in channels [8*(o/8), 8*(o/8) + 8)) -> mean = channels 0..11, logvar = channels 12..23 (the reference's
+// reshape (B, 8, 3, H, W) + chunk(2, dim=1): latent channel j = c*3 + n is conv channel j, its logvar conv channel
+// 12 + j) -> soft clamp 20*tanh(lv/20) -> std = exp(0.5*lv) -> z = mean + std*noise.  The three outputs are written in
+// the (B, 12, S, S) layout, consecutive threads on consecutive pixels.
+__global__ void __launch_bounds__(256)
+vae_posterior_kernel(const ln3_vae_posterior_args a) {
+  __shared__ float s_w[24 * 8 + 24];
+  for (int i = threadIdx.x; i < 24 * 8; i += blockDim.x) s_w[i] = a.w[i];
+  if (threadIdx.x < 24) s_w[24 * 8 + threadIdx.x] = a.bias[threadIdx.x];
+  __syncthreads();
+  const int L = a.S * a.S;
+  const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (idx >= static_cast<long long>(a.B) * L) return;
+  const int b = static_cast<int>(idx / L), l = static_cast<int>(idx % L);
+  float h[24];
+  const float* hp = a.moments + idx * 24;
+#pragma unroll
+  for (int c = 0; c < 24; ++c) h[c] = __ldg(hp + c);
+  const long long obase = static_cast<long long>(b) * 12 * L + l;
+#pragma unroll
+  for (int j = 0; j < 12; ++j) {
+    float m = 0.f, lv = 0.f;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+      m = fmaf(s_w[j * 8 + k], h[(j / 8) * 8 + k], m);
+      lv = fmaf(s_w[(12 + j) * 8 + k], h[((12 + j) / 8) * 8 + k], lv);
+    }
+    m = __fadd_rn(m, s_w[192 + j]);
+    lv = __fadd_rn(lv, s_w[192 + 12 + j]);
+    // torch: logvar.div(20.).tanh().mul(20.); std = exp(0.5 * logvar); mean + std * randn -- one rounding per op
+    lv = __fmul_rn(tanhf(__fdiv_rn(lv, 20.f)), 20.f);
+    const long long o = obase + static_cast<long long>(j) * L;
+    a.mean[o] = m;
+    a.logvar[o] = lv;
+    a.z[o] = a.noise ? __fadd_rn(m, __fmul_rn(expf(__fmul_rn(0.5f, lv)), a.noise[o])) : m;
+  }
+}
+
+int vae_posterior(const ln3_vae_posterior_args* a, cudaStream_t stream) {
+  if (a->B < 0 || a->S <= 0) return set_error(LN3_EINVAL, "vae_posterior: need B >= 0 and S > 0");
+  if (!a->moments || !a->w || !a->bias || !a->mean || !a->logvar || !a->z)
+    return set_error(LN3_EINVAL, "vae_posterior: null pointer (only noise may be NULL)");
+  if (a->B == 0) return LN3_OK;
+  const long long n = static_cast<long long>(a->B) * a->S * a->S;
+  if ((n + 255) / 256 > 0x7fffffffLL) return set_error(LN3_EINVAL, "vae_posterior: B*S*S too large");
+  vae_posterior_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, stream>>>(*a);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return set_error(LN3_ECUDA, "vae_posterior launch: %s", cudaGetErrorString(e));
   count_launch();
   return LN3_OK;
 }

@@ -92,5 +92,7 @@ int attn_single_head(const float* q, const float* k, const float* v, float* out,
                      cudaStream_t stream);
 int patch_embed_triplane(const float* x, const float* w, const float* bias, int B, int Cz, int S, int E,
                          float in_mul, float* tokens, void* silu_bf16, cudaStream_t stream);
+int downsample_nhwc(const ln3_conv_args* a, cudaStream_t stream);
+int vae_posterior(const ln3_vae_posterior_args* a, cudaStream_t stream);
 
 }  // namespace ln3

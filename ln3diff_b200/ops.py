@@ -537,6 +537,55 @@ def conv_nhwc(x: torch.Tensor, w_packed: torch.Tensor, bias: torch.Tensor | None
     return out
 
 
+def downsample_nhwc(x: torch.Tensor, w_packed: torch.Tensor, bias: torch.Tensor | None, *,
+                    out: torch.Tensor | None = None, tf32: bool = False) -> torch.Tensor:
+    """The encoder's Downsample: 3x3 conv, stride 2, on F.pad(x, (0,1,0,1)).  x (N,H,W,Cin) NHWC fp32 with H, W
+    even; w_packed (9, Cin, Cout); returns (N, H/2, W/2, Cout).  tf32=True: TF32 operands, fp32 accumulate."""
+    _cuda(x, "x", torch.float32)
+    _cuda(w_packed, "w_packed", torch.float32)
+    _req(x.dim() == 4 and x.is_contiguous() and w_packed.dim() == 3 and w_packed.is_contiguous(), "bad conv operands")
+    N, H, W, Cin = x.shape
+    _req(H % 2 == 0 and W % 2 == 0, "downsample needs even H, W")
+    _req(w_packed.shape[0] == 9 and w_packed.shape[1] == Cin, "weight must be (9, Cin, Cout)")
+    Cout = w_packed.shape[2]
+    if out is None:
+        out = torch.empty((N, H // 2, W // 2, Cout), device=x.device, dtype=torch.float32)
+    _cuda(out, "out", torch.float32)
+    _req(out.shape == (N, H // 2, W // 2, Cout) and out.is_contiguous(), "bad out")
+    a = _lib.ConvArgs()
+    a.x, a.w, a.out = x.data_ptr(), w_packed.data_ptr(), out.data_ptr()
+    if bias is not None:
+        _cuda(bias, "bias", torch.float32)
+        _req(bias.shape == (Cout,) and bias.is_contiguous(), "bias must be contiguous (Cout,)")
+        a.bias = bias.data_ptr()
+    a.N, a.H, a.W, a.Cin, a.Cout, a.ksize = N, H, W, Cin, Cout, 3
+    a.precision = _lib.MLP_TF32 if tf32 else _lib.MLP_FP32
+    _lib.check(_lib.lib().ln3_downsample_nhwc(C.byref(a), _lib.current_stream()), "ln3_downsample_nhwc")
+    return out
+
+
+def vae_posterior(moments: torch.Tensor, w: torch.Tensor, bias: torch.Tensor, noise: torch.Tensor | None = None):
+    """moments (B,S,S,24) NHWC fp32 -> (mean, logvar, z), each (B,12,S,S) fp32: quant_conv (w (24,8), bias (24,)),
+    the soft-clamped logvar and z = mean + exp(0.5 logvar) * noise (noise (B,12,S,S), or None for z = mean)."""
+    _cuda(moments, "moments", torch.float32)
+    _req(moments.dim() == 4 and moments.shape[3] == 24 and moments.shape[1] == moments.shape[2]
+         and moments.is_contiguous(), "moments must be contiguous (B,S,S,24)")
+    B, S = moments.shape[0], moments.shape[1]
+    for nm, t_, shp in (("w", w, (24, 8)), ("bias", bias, (24,))):
+        _cuda(t_, nm, torch.float32)
+        _req(tuple(t_.shape) == shp and t_.is_contiguous(), f"{nm} must be contiguous {shp}")
+    mean, logvar, z = (torch.empty((B, 12, S, S), device=moments.device, dtype=torch.float32) for _ in range(3))
+    a = _lib.VaePosteriorArgs()
+    if noise is not None:
+        _cuda(noise, "noise", torch.float32)
+        _req(noise.shape == (B, 12, S, S) and noise.is_contiguous(), "noise must be contiguous (B,12,S,S)")
+        a.noise = noise.data_ptr()
+    a.moments, a.w, a.bias = moments.data_ptr(), w.data_ptr(), bias.data_ptr()
+    a.mean, a.logvar, a.z, a.B, a.S = mean.data_ptr(), logvar.data_ptr(), z.data_ptr(), B, S
+    _lib.check(_lib.lib().ln3_vae_posterior(C.byref(a), _lib.current_stream()), "ln3_vae_posterior")
+    return mean, logvar, z
+
+
 def groupnorm_stats(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, groups: int = 32,
                     eps: float = 1e-6):
     """x (N,H,W,C) fp32 NHWC -> per-(image, channel) (scale, shift) of GroupNorm(groups, C, eps)."""

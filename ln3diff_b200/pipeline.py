@@ -247,6 +247,33 @@ def image_to_3d(conditioner, model, decoder, image: torch.Tensor, cameras: torch
                        num_steps, cfg_scale, sampling_method, resolution, dtype)
 
 
+@torch.no_grad()
+def encode_latents(encoder, decoder, img_to_encoder: torch.Tensor, sample_posterior: bool = True) -> dict:
+    """`AE.forward(img=img_to_encoder, behaviour='encoder_vae')` (nsr/script_util.py:326-329), the first step of
+    `eval_novelview_loop` (nsr/train_nv_util.py:1177-1219): img_to_encoder (B*4, 10, 256, 256) fp32 -- per view RGB in
+    [-1, 1], the Plücker rays o x d and d, and depth -- through MVEncoder to the moments (B, 24, 32, 32), then the
+    decoder's vae_reparameterization.  Returns the reference's dict; `latent_normalized_2Ddiffusion` (B, 12, 32, 32) is
+    the latent every stage-2 DiT is trained on (what `--save_latent True` writes).  sample_posterior draws the noise
+    from the CPU generator, as the reference does."""
+    if not img_to_encoder.is_cuda:
+        raise RuntimeError("encode_latents runs on CUDA only (no CPU fallback)")
+    return decoder.vae_reparameterization(encoder(img_to_encoder), sample_posterior)
+
+
+@torch.no_grad()
+def reconstruct(encoder, decoder, img_to_encoder: torch.Tensor, cameras: torch.Tensor, resolution: int = 128,
+                scaling_divider: float = 1.0, sample_posterior: bool = True, noise: tuple | None = None,
+                mlp_tf32: bool = True):
+    """3D reconstruction from multi-view images, the body of `eval_novelview_loop`: `encode_latents`, then decode and
+    render of every camera of `cameras` (V, 25) for every object.  The reconstruction trainer renders the posterior
+    latent with `triplane_scaling_divider = 1.0` (TrainLoop3DRec, nsr/train_util.py:565, applied at :580).
+    Returns (the encoder_vae dict, the render dict of `decode_and_render`)."""
+    ret = encode_latents(encoder, decoder, img_to_encoder, sample_posterior)
+    out = decode_and_render(decoder, ret["latent_normalized_2Ddiffusion"], cameras, resolution,
+                            scaling_divider=scaling_divider, noise=noise, mlp_tf32=mlp_tf32)
+    return ret, out
+
+
 # ---------------------------------------------------------------------------------------------- multi-GPU
 def shard_range(n_total: int, world: int, rank: int) -> tuple[int, int, int]:
     """Contiguous block of ceil(P/G) prompts per rank (SURVEY.md section 8e): returns (lo, hi, per) with

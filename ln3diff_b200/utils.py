@@ -129,3 +129,20 @@ def build_ae_decoder(arch: str = "DiT2-L/2", image_size: int = 128, seed: int = 
     derandomize_zero_init(m)
     m.eval()
     return m.to(device) if device else m
+
+
+def build_ae_encoder(seed: int = 0, device: str | None = None, ch: int = 64, num_res_blocks: int = 1,
+                     in_channels: int = 10):
+    """The stage-1 encoder as create_3DAE_model builds it for dino_version 'mv-sd-dit' (nsr/script_util.py:1294-1339)
+    with the release scripts' sd_E_ch=64, sd_E_num_res_blocks=1: MVEncoder(double_z=True, resolution=256,
+    in_channels=10, ch_mult=[1,2,4,4], z_channels=12, attn_kwargs={'n_heads': 8, 'd_head': 64}).  Random init; the
+    zero-initialised proj_out of the mid-block transformer is re-randomised (derandomize_zero_init), otherwise the
+    whole transformer would be multiplied by zero."""
+    from .ldm.modules.diffusionmodules.model import MVEncoder
+    torch.manual_seed(seed)
+    m = MVEncoder(double_z=True, resolution=256, in_channels=in_channels, ch=ch, ch_mult=[1, 2, 4, 4],
+                  num_res_blocks=num_res_blocks, num_frames=4, dropout=0.0, attn_resolutions=[], out_ch=3,
+                  z_channels=12, attn_kwargs={"n_heads": 8, "d_head": 64})
+    derandomize_zero_init(m)
+    m.eval()
+    return m.to(device) if device else m

@@ -11,6 +11,8 @@ per block), NHWC fp32 conv kernels for the SD decoder.  The DiT2 token stream is
 in place (tokens are NHWC) and conv_out writes the channels-last tri-plane the ray marcher reads."""
 from __future__ import annotations
 
+import math
+
 import torch
 import torch.nn as nn
 
@@ -29,6 +31,56 @@ class PatchEmbedTriplane(nn.Module):
         self.img_size, self.patch_size = (img_size, img_size), (patch_size, patch_size)
         self.num_patches = (img_size // patch_size) ** 2
         self.proj = nn.Conv2d(in_chans, embed_dim * 3, kernel_size=patch_size, stride=patch_size, bias=bias, groups=3)
+
+
+class DiagonalGaussianDistribution:
+    """utils/torch_utils/distributions/distributions.py:29-113: the VAE posterior over the tri-plane latent.
+    mean / logvar are (B, z, 3, L); logvar is soft-clamped to 20 tanh(lv / 20) when soft_clamp (the release setting).
+    `sample()` draws its noise from the CPU generator, `torch.randn(mean.shape)`, and moves it to the device, exactly as
+    the reference does, so the same `torch.manual_seed` gives the same latent on any device."""
+
+    def __init__(self, parameters, deterministic=False, soft_clamp=False):
+        self.parameters = parameters
+        self.mean, logvar = torch.chunk(parameters, 2, dim=1)
+        self.logvar = logvar.div(20.0).tanh().mul(20.0) if soft_clamp else torch.clamp(logvar, -30.0, 20.0)
+        self.deterministic = deterministic
+        self._finish()
+
+    @classmethod
+    def from_kernel(cls, mean, logvar):
+        """The posterior whose mean and (already clamped) logvar ln3_vae_posterior wrote."""
+        self = cls.__new__(cls)
+        self.parameters, self.mean, self.logvar, self.deterministic = None, mean, logvar, False
+        self._finish()
+        return self
+
+    def _finish(self):
+        self.std = torch.exp(0.5 * self.logvar)
+        self.var = torch.exp(self.logvar)
+        if self.deterministic:
+            self.var = self.std = torch.zeros_like(self.mean)
+
+    def sample(self):
+        return self.mean + self.std * torch.randn(self.mean.shape).to(device=self.mean.device)
+
+    def mode(self):
+        return self.mean
+
+    def log_p(self, samples):
+        # the reference divides by var, not std (distributions.py:72-78); kept
+        normalized_samples = (samples - self.mean) / self.var
+        return -0.5 * normalized_samples * normalized_samples - 0.5 * math.log(2 * math.pi) - self.logvar
+
+    def normal_entropy(self):
+        return self.logvar + 0.5 * (math.log(2 * math.pi) + 1)
+
+    def kl(self, other=None):
+        if self.deterministic:
+            return torch.Tensor([0.0])
+        if other is None:
+            return 0.5 * torch.sum(torch.pow(self.mean, 2) + self.var - 1.0 - self.logvar, dim=[1, 2, 3])
+        return 0.5 * torch.sum(torch.pow(self.mean - other.mean, 2) / other.var + self.var / other.var - 1.0
+                               - self.logvar + other.logvar, dim=[1, 2, 3])
 
 
 class RodinSR_256_fusionv6_ConvQuant_liteSR_dinoInit3DAttn_SD_B_3L_C_withrollout_withSD_D_ditDecoder(nn.Module):
@@ -52,6 +104,8 @@ class RodinSR_256_fusionv6_ConvQuant_liteSR_dinoInit3DAttn_SD_B_3L_C_withrollout
                             attn_resolutions=[], out_ch=32, z_channels=D)))
         self.decoder_pred = None
         self.D_roll_out_input = False
+        self.plane_n = 3
+        self.reparameterization_soft_clamp = True
         self._prep = None
 
     # ------------------------------------------------------------------ weight repack
@@ -91,6 +145,8 @@ class RodinSR_256_fusionv6_ConvQuant_liteSR_dinoInit3DAttn_SD_B_3L_C_withrollout
             return d
 
         at = sr.mid.attn_1
+        qc = self.superresolution["quant_conv"]
+        P["quant"] = (f32(qc.weight.reshape(qc.weight.shape[0], -1)), f32(qc.bias))
         P["sr"] = dict(conv_in=pk(sr.conv_in), mid1=res(sr.mid.block_1), mid2=res(sr.mid.block_2),
                        attn=dict(n=(f32(at.norm.weight), f32(at.norm.bias)), q=pk(at.q), k=pk(at.k), v=pk(at.v),
                                  o=pk(at.proj_out)),
@@ -179,6 +235,48 @@ class RodinSR_256_fusionv6_ConvQuant_liteSR_dinoInit3DAttn_SD_B_3L_C_withrollout
         out = ops.conv_nhwc(h, *S["conv_out"], ksize=3, gn=ops.groupnorm_stats(h, *S["nout"]), swish=True, tf32=tf)
         return out.view(B, 3, out.shape[1], out.shape[2], out.shape[3])
 
+    # ------------------------------------------------------------------ VAE posterior (encoder side)
+    @torch.no_grad()
+    def _posterior(self, moments, sample_posterior: bool):
+        """moments (B, 24, S, S) -> (posterior, latent (B, 4, 3, S*S)) on ln3_vae_posterior.  A channels-last view (what
+        the encoder mirror returns) reaches the kernel without a copy."""
+        if not moments.is_cuda:
+            raise RuntimeError("ln3diff_b200 decoder runs on CUDA only (no CPU fallback)")
+        assert self.reparameterization_soft_clamp and self.plane_n == 3 and self.vae_p > 1
+        if self._prep is None:
+            self.prepare()
+        B, C2, H, W = moments.shape
+        assert C2 == 6 * self.ldm_z_channels == 24 and H == W, "moments must be (B, 24, S, S)"
+        nhwc = moments.float().permute(0, 2, 3, 1).contiguous()
+        # sample(): the CPU generator's randn(mean.shape), as the reference draws it
+        noise = torch.randn(B, 12, H, W).to(moments.device) if sample_posterior else None
+        mean, logvar, z = ops.vae_posterior(nhwc, *self._prep["quant"], noise)
+        shp = (B, self.ldm_z_channels, self.plane_n, H * W)          # the reference's (B, C, 3, L)
+        return DiagonalGaussianDistribution.from_kernel(mean.view(shp), logvar.view(shp)), z.view(shp)
+
+    def vae_encode(self, h):
+        """vit_triplane.py:912-933: quant_conv + DiagonalGaussianDistribution(soft_clamp=True) of the encoder moments."""
+        return self._posterior(h, False)[0]
+
+    def vae_reparameterization(self, latent, sample_posterior):
+        """vit_triplane.py:1152-1199: encoder moments (B, 24, 32, 32) -> the reference's dict (posterior sample or mode,
+        log_q with its division by var, the (B, 12, 32, 32) diffusion latent)."""
+        posterior, latent = self._posterior(latent, sample_posterior)
+        log_q = posterior.log_p(latent)
+        S = self.token_size * self.vae_p
+        B = latent.shape[0]
+        return dict(normal_entropy=posterior.normal_entropy(),
+                    latent_normalized=latent.permute(0, 2, 3, 1).reshape(B, -1, latent.shape[1]),
+                    latent_normalized_2Ddiffusion=latent.reshape(B, -1, S, S),
+                    log_q_2Ddiffusion=log_q.reshape(B, -1, S, S),
+                    log_q=log_q,
+                    posterior=posterior)
+
+    def vit_decode(self, latent, img_size, sample_posterior=True, **kwargs):
+        """vit_triplane.py:879-885: reparameterise the encoder moments, then decode to the tri-plane."""
+        ret_dict = self.vae_reparameterization(latent, sample_posterior)
+        return self.vit_decode_postprocess(self.vit_decode_backbone(ret_dict, img_size), ret_dict)
+
     # ------------------------------------------------------------------ reference-named entry points
     def vit_decode_backbone(self, latent, img_size=None):
         """Returns a handle consumed by vit_decode_postprocess (the fused decode runs there)."""
@@ -245,3 +343,9 @@ class RodinSR_256_fusionv6_ConvQuant_liteSR_dinoInit3DAttn_SD_B_3L_C_withrollout
         G = grid_size
         return {"rgb": rgb.reshape(N, G, G, G, -1), "sigma": sigma.reshape(N, G, G, G, -1)}
 
+
+
+# `vae_reconstruction.sh` names the `_S` variant (vit_triplane.py:1517-1837).  Its decode and reparameterisation compute
+# what the class above computes and its state_dict has the same keys and shapes (DiT2-B/2 and DiT2-L/2).
+RodinSR_256_fusionv6_ConvQuant_liteSR_dinoInit3DAttn_SD_B_3L_C_withrollout_withSD_D_ditDecoder_S = \
+    RodinSR_256_fusionv6_ConvQuant_liteSR_dinoInit3DAttn_SD_B_3L_C_withrollout_withSD_D_ditDecoder
