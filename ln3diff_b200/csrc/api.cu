@@ -41,6 +41,19 @@ int device_sm_count() {
   return n;
 }
 
+int device_l2_bytes() {
+  static std::atomic<int> l2[64];   // per device ordinal; 0 = not queried yet
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess) return 0;
+  std::atomic<int>& slot = l2[dev & 63];
+  int n = slot.load(std::memory_order_relaxed);
+  if (n == 0) {
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrL2CacheSize, dev) != cudaSuccess || n <= 0) n = 0;
+    slot.store(n, std::memory_order_relaxed);
+  }
+  return n;
+}
+
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*,
                                   const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
                                   const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,

@@ -62,6 +62,7 @@ struct GemmParams {
   int hn_nsec, hn_sec_cols;
   float hn_eps;
   int tma_store;           // bf16 output through the staging tile and tensor map (ldo % 8 == 0), else direct stores
+  int n_first;             // tile walk: N first across the whole width, else M first inside each N panel
 };
 
 template <int ACT>
@@ -193,8 +194,8 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int tiles_m = (p.M + BM - 1) / BM;
-  const int num_tiles = tiles_m * (p.N / BN);
+  const int tiles_m = (p.M + BM - 1) / BM, tiles_n = p.N / BN;
+  const int num_tiles = tiles_m * tiles_n;
   const int num_kb = p.K / BK;
 
   if (threadIdx.x == 0) {
@@ -211,13 +212,24 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   pdl_wait();  // barrier set-up and descriptor prefetch overlapped the previous kernel
 
   // Tile order: consecutive CTAs walk M first inside an N panel, so the concurrently resident tiles share
-  // W panels (L2 reuse) while A panels stream.
+  // W panels (L2 reuse) while A panels stream.  With p.n_first they walk N first across the whole width instead:
+  // when A does not fit in the L2, each A panel is then read from memory once rather than once per N panel.
+  auto tile_of = [&](int t, int& tm, int& tn) {
+    if (p.n_first) {
+      tm = t / tiles_n;
+      tn = t % tiles_n;
+    } else {
+      tm = t % tiles_m;
+      tn = t / tiles_m;
+    }
+  };
   if (warp >= 8) {
     if (warp == 8 && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
       for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-        const int tm = t % tiles_m, tn = t / tiles_m;
+        int tm, tn;
+        tile_of(t, tm, tn);
         for (int kb = 0; kb < num_kb; ++kb) {
           mbar_wait_silent(&empty_bar[stage], phase ^ 1);
           mbar_arrive_expect_tx(&full_bar[stage], kStageBytes);
@@ -250,7 +262,8 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   uint8_t* stage_out = staged ? smem_out + wg * kOutStageBytes : nullptr;
   float acc0[BN / 2], acc1[BN / 2];  // rows [0, 64) and [64, 128) of the tile
   for (int t = blockIdx.x + wg * grid; t < num_tiles; t += 2 * grid) {
-    const int tm = t % tiles_m, tn = t / tiles_m;
+    int tm, tn;
+    tile_of(t, tm, tn);
     if (t >= 2 * grid || wg == 1) named_bar_sync(kOrderBar + wg, 256);
     uint32_t stage = slot % kStages, phase = (slot / kStages) & 1;
     uint32_t prev_stage = 0;
@@ -379,6 +392,9 @@ int gemm_bf16(const ln3_gemm_args* a, cudaStream_t stream) {
   p.hn_sec_cols = a->head_norm_sec_cols;
   p.hn_eps = a->head_norm_eps;
   p.tma_store = tma_store ? 1 : 0;
+  // N-first walk when A does not fit in the L2 but W fits in half of it (the MLP's fc2: a 100 MB A, an 8 MB W)
+  const long long l2 = device_l2_bytes();
+  p.n_first = 2LL * a->M * a->K > l2 && 2LL * a->N * a->K <= l2 / 2;
   if (a->head_norm_w != nullptr) {
     if (a->out_kind != LN3_OUT_BF16 || a->act != LN3_ACT_NONE)
       return set_error(LN3_EINVAL, "gemm: head_norm needs LN3_OUT_BF16 and no activation");

@@ -14,6 +14,7 @@ namespace ln3 {
 int set_error(int code, const char* fmt, ...);
 void count_launch(int n = 1);
 int device_sm_count();
+int device_l2_bytes();
 // Per-device one-shot guard.  cudaFuncSetAttribute(MaxDynamicSharedMemorySize) and the SM count belong to
 // the device that is current at the call; one process may drive several GPUs and two host threads may race
 // the first call, so "done" is tracked per device ordinal (bit d of a mask) under a mutex.

@@ -2,13 +2,14 @@
 
     python tools/gemm_shapes.py [--lib PATH [--lib PATH ...]] [--rounds R] [--window-s S]
 
-The six shapes are the per-layer GEMMs of `dit/dit_trilatent.py::_forward_impl` at bench.py's batch (8 prompts
+The first six shapes are the per-layer GEMMs of `dit/dit_trilatent.py::_forward_impl` at bench.py's batch (8 prompts
 with CFG = 16 samples of 768 tokens, D = 1024), each with its production epilogue; fc1 runs the default
-erf-GELU.  The yardstick is `torch.nn.functional.linear` in bf16 (cuBLAS), with `F.gelu` applied separately
-for fc1.  Every entry is timed with CUDA events over enough back-to-back launches to fill a window of
+erf-GELU.  The last is the CLIP text tower's qkv for 8 prompts (616 rows, a small GEMM of partial tiles).  The
+yardstick is `torch.nn.functional.linear` in bf16 (cuBLAS), with `F.gelu` applied separately for fc1.  Every entry is timed with CUDA events over enough back-to-back launches to fill a window of
 `--window-s` seconds, after a warm-up.  Several `--lib` builds of libln3b200.so are timed alternately in one
-process on the same inputs, `--rounds` times each, so that two builds can be compared under the same clocks.
-Prints one line per (round, build, shape) and a final JSON line with the card name, power limit and the median SM
+process on the same inputs, `--rounds` times each, so that two builds can be compared under the same clocks; the
+outputs of every build are compared with the first build's, bit for bit (max abs and rel-L2 difference when they
+are not identical).  Prints one line per (round, build, shape) and a final JSON line with the card name, power limit and the median SM
 clock sampled during the run.  Needs a GPU; it is a measurement, not a test.
 """
 from __future__ import annotations
@@ -34,6 +35,7 @@ SHAPES = [
     ("cross_out", MH, D, D, True, "none"),
     ("fc1", M, 4 * D, D, True, "gelu_erf"),
     ("fc2", M, D, 4 * D, True, "none"),
+    ("clip_qkv", 8 * 77, 3 * 768, 768, True, "none"),
 ]
 
 
@@ -133,12 +135,34 @@ def main() -> None:
             return lambda: F.gelu(F.linear(a, w, bb))
         return lambda: F.linear(a, w, bb)
 
+    # bit-identity of every build's outputs against the first build's (same inputs, one launch each)
+    ref_out, diffs = {}, []
+    for lib in libs:
+        _lib._lib, _lib.LIB_PATH = None, Path(lib)     # ops.gemm resolves the library on every call
+        for sname, *_, act in SHAPES:
+            out = inputs[sname][3]
+            out.fill_(0)
+            ours(sname, act)()
+            torch.cuda.synchronize()
+            o = out.clone()
+            if sname not in ref_out:
+                ref_out[sname] = o
+                continue
+            r = ref_out[sname]
+            same = torch.equal(o.view(torch.int16), r.view(torch.int16))
+            d = o.float() - r.float()
+            row = {"impl": lib, "shape": sname, "bit_identical": same, "max_abs": d.abs().max().item(),
+                   "rel_l2": (d.norm() / r.float().norm()).item()}
+            diffs.append(row)
+            print(f"compare {sname:10s} bit-identical={same} max_abs={row['max_abs']:.3e} "
+                  f"rel_l2={row['rel_l2']:.3e}  {lib}", flush=True)
+
     clock = ClockPoll()
     rows = []
     try:
         for r in range(args.rounds):
             for lib in libs:
-                _lib._lib, _lib.LIB_PATH = None, Path(lib)     # ops.gemm resolves the library on every call
+                _lib._lib, _lib.LIB_PATH = None, Path(lib)
                 for sname, m, n, k, _, act in SHAPES:
                     ms = time_window(torch, ours(sname, act), args.window_s)
                     tf = 2.0 * m * n * k / (ms / 1e3) / 1e12
@@ -156,7 +180,7 @@ def main() -> None:
     finally:
         sm_mhz = clock.stop()
     print(json.dumps({"gpu": name, "power_limit_w": float(power_limit), "sm_mhz_median": sm_mhz,
-                      "window_s": args.window_s, "rows": rows}), flush=True)
+                      "window_s": args.window_s, "compare": diffs, "rows": rows}), flush=True)
 
 
 if __name__ == "__main__":
