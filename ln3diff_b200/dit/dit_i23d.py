@@ -16,13 +16,11 @@ from __future__ import annotations
 import torch
 import torch.nn as nn
 
-from .. import _lib, ops
+from .. import ops
 from .._lib import NORM_LAYER, NORM_NONE, NORM_RMS
-from ._pixart import PixArtGraphMixin
-from .dit_trilatent import _attention_rows
+from ._denoiser import PixArtMixin, cross_attention_context, split_kv
 from .dit_models_xformers import (Attention, CaptionEmbedder, MemoryEfficientCrossAttention, T2IFinalLayer,
-                                  TimestepEmbedder, _FusedMLP, _PatchEmbed, _RMSNormParam,
-                                  get_2d_sincos_pos_embed)
+                                  TimestepEmbedder, _FusedMLP, _PatchEmbed, _RMSNormParam)
 
 
 class ImageCondDiTBlockPixelArtRMSNorm(nn.Module):
@@ -48,8 +46,7 @@ class ImageCondDiTBlockPixelArtRMSNormNoClip(ImageCondDiTBlockPixelArtRMSNorm):
     its forward runs self-attention over the latent tokens only and cross-attends the multi-view DINO tokens."""
 
 
-class DiT_I23D_PixelArt(PixArtGraphMixin, nn.Module):
-    _ln3_fused_in_scale = False
+class DiT_I23D_PixelArt(PixArtMixin, nn.Module):
     _vit_blk = ImageCondDiTBlockPixelArtRMSNorm
 
     def __init__(self, input_size=32, patch_size=2, in_channels=4, hidden_size=1152, depth=28, num_heads=16,
@@ -85,65 +82,9 @@ class DiT_I23D_PixelArt(PixArtGraphMixin, nn.Module):
         self._invalidate()
 
     def initialize_weights(self):
-        def _basic_init(m):
-            if isinstance(m, nn.Linear):
-                nn.init.xavier_uniform_(m.weight)
-                if m.bias is not None:
-                    nn.init.constant_(m.bias, 0)
-        self.apply(_basic_init)
-        w = self.x_embedder.proj.weight.data
-        nn.init.xavier_uniform_(w.view([w.shape[0], -1]))
-        nn.init.constant_(self.x_embedder.proj.bias, 0)
-        nn.init.normal_(self.t_embedder.mlp[0].weight, std=0.02)
-        nn.init.normal_(self.t_embedder.mlp[2].weight, std=0.02)
-        nn.init.constant_(self.final_layer.linear.weight, 0)
-        nn.init.constant_(self.final_layer.linear.bias, 0)
-        nn.init.constant_(self.adaLN_modulation[-1].weight, 0)
-        nn.init.constant_(self.adaLN_modulation[-1].bias, 0)
-        nn.init.constant_(self.cap_embedder[-1].weight, 0)
-        nn.init.constant_(self.cap_embedder[-1].bias, 0)
-        p = int(self.x_embedder.num_patches ** 0.5)
-        D = self.pos_embed.shape[-1]
-        pe = get_2d_sincos_pos_embed(D, (3, p * p)).reshape(3 * p * p, D)
-        self.pos_embed.data.copy_(torch.from_numpy(pe).float().unsqueeze(0))
+        super().initialize_weights([self.adaLN_modulation[-1], self.cap_embedder[-1]])
 
-    @torch.no_grad()
-    def prepare(self):
-        dev = self.pos_embed.device
-        if dev.type != "cuda":
-            raise RuntimeError("ln3diff_b200 DiT runs on CUDA only (no CPU fallback)")
-        bf = lambda w: w.detach().to(dev, torch.bfloat16).contiguous()
-        f32 = lambda w: w.detach().to(dev, torch.float32).contiguous()
-        D = self.embed_dim
-        P = dict(t0_w=bf(self.t_embedder.mlp[0].weight), t0_b=f32(self.t_embedder.mlp[0].bias),
-                 t2_w=bf(self.t_embedder.mlp[2].weight), t2_b=f32(self.t_embedder.mlp[2].bias),
-                 ada_w=bf(self.adaLN_modulation[1].weight), ada_b=f32(self.adaLN_modulation[1].bias),
-                 pe_w=f32(self.x_embedder.proj.weight), pe_b=f32(self.x_embedder.proj.bias), pos=f32(self.pos_embed),
-                 fin_w=f32(self.final_layer.linear.weight), fin_b=f32(self.final_layer.linear.bias),
-                 fin_tab=f32(self.final_layer.scale_shift_table),
-                 tables=f32(torch.stack([b.scale_shift_table.detach().reshape(-1) for b in self.blocks], 0)),
-                 **self._prepare_context_weights(bf, f32))
-        blocks = []
-        for b in self.blocks:
-            qkv_w, qkv_b = b.attn.qkv.weight.detach(), b.attn.qkv.bias.detach()
-            blocks.append(dict(
-                n1_w=f32(b.norm1.weight), n2_w=f32(b.norm2.weight),
-                qkv_w=bf(qkv_w), qkv_b=f32(qkv_b),
-                qk_norm=f32(torch.stack([b.attn.q_norm.weight.detach(), b.attn.k_norm.weight.detach()], 0)),
-                **self._prepare_block_context_weights(b, bf, f32),
-                proj_w=bf(b.attn.proj.weight), proj_b=f32(b.attn.proj.bias),
-                cq_w=bf(b.cross_attn.to_q.weight), cq_norm=f32(b.cross_attn.q_norm.weight.detach()[None]),
-                ckv_w=bf(torch.cat([b.cross_attn.to_k.weight.detach(), b.cross_attn.to_v.weight.detach()], 0)),
-                ck_norm=f32(b.cross_attn.k_norm.weight.detach()[None]),
-                co_w=bf(b.cross_attn.to_out[0].weight), co_b=f32(b.cross_attn.to_out[0].bias),
-                fc1_w=bf(b.mlp.mlp[0].weight), fc1_b=f32(b.mlp.mlp[1].bias),
-                fc2_w=bf(b.mlp.mlp[2].weight), fc2_b=f32(b.mlp.mlp[3].bias)))
-        P["blocks"] = blocks
-        self._invalidate()
-        self._prep = P
-        return P
-
-    def _prepare_context_weights(self, bf, f32) -> dict:
+    def _pack_context(self, bf, f32) -> dict:
         """Model-level weights of the conditioning: cap_embedder, attention_y_norm, dino_proj."""
         return dict(cap_ln_w=f32(self.cap_embedder[0].weight), cap_ln_b=f32(self.cap_embedder[0].bias),
                     cap_w=bf(self.cap_embedder[1].weight), cap_b=f32(self.cap_embedder[1].bias),
@@ -151,7 +92,15 @@ class DiT_I23D_PixelArt(PixArtGraphMixin, nn.Module):
                     d1_w=bf(self.dino_proj.y_proj.fc1.weight), d1_b=f32(self.dino_proj.y_proj.fc1.bias),
                     d2_w=bf(self.dino_proj.y_proj.fc2.weight), d2_b=f32(self.dino_proj.y_proj.fc2.bias))
 
-    def _prepare_block_context_weights(self, b, bf, f32) -> dict:
+    def _pack_block(self, b, bf, f32) -> dict:
+        return dict(n1_w=f32(b.norm1.weight), n2_w=f32(b.norm2.weight),
+                    qk_norm=f32(torch.stack([b.attn.q_norm.weight.detach(), b.attn.k_norm.weight.detach()], 0)),
+                    cq_norm=f32(b.cross_attn.q_norm.weight.detach()[None]),
+                    ckv_w=bf(torch.cat([b.cross_attn.to_k.weight.detach(), b.cross_attn.to_v.weight.detach()], 0)),
+                    ck_norm=f32(b.cross_attn.k_norm.weight.detach()[None]),
+                    **self._pack_dino_block(b, bf, f32))
+
+    def _pack_dino_block(self, b, bf, f32) -> dict:
         """Per-block K|V rows of the qkv projection (and the k_norm) for the DINO tokens of self-attention."""
         D = self.embed_dim
         return dict(kv_w=bf(b.attn.qkv.weight[D:]), kv_b=f32(b.attn.qkv.bias[D:]),
@@ -162,6 +111,7 @@ class DiT_I23D_PixelArt(PixArtGraphMixin, nn.Module):
         """Step-invariant conditioning, once per prompt batch: pooled-CLIP embedding, per-layer
         cross-attention K/V of the RMS-normed CLIP tokens, per-layer self-attention K/V of the
         projected DINO tokens."""
+        assert isinstance(context, dict)
         vec0, ca0 = vec, ca = context["vector"], context["crossattn"]
         hit = self._ctx_cache.get(vec0, ca0)
         if hit is not None:
@@ -176,7 +126,6 @@ class DiT_I23D_PixelArt(PixArtGraphMixin, nn.Module):
             dkv=torch.empty(self.depth, B, Lc, 2 * D, device=dev, dtype=torch.bfloat16),
             oc=torch.empty(self.depth, B, D, device=dev, dtype=torch.bfloat16)))
         vec = vec.float().contiguous()
-        ones = torch.ones(1, device=dev)
         # cap_embedder: LayerNorm(affine, eps 1e-5) -> Linear.  LN(x)*w + b == LN(x)*(1 + (w-1)) + b
         vn = ops.norm_modulate(vec, norm=NORM_LAYER, eps=1e-5, shift=P["cap_ln_b"][None], scale=(P["cap_ln_w"] - 1)[None],
                                mod_rows=B)
@@ -189,37 +138,9 @@ class DiT_I23D_PixelArt(PixArtGraphMixin, nn.Module):
         for l, W in enumerate(P["blocks"]):
             ops.gemm(clip, W["ckv_w"], out=ckv[l].view(B * Lc, 2 * D), head_norm=W["ck_norm"], head_norm_sec_cols=D)
             ops.gemm(dino, W["kv_w"], W["kv_b"], out=dkv[l].view(B * Lc, 2 * D), head_norm=W["k_norm"], head_norm_sec_cols=D)
-        out = dict(cls=cls, ckv=ckv, dkv=dkv, rows=(0, B), oconst=None)
-        # identical CLIP tokens (the all-zero unconditional half of forward_with_cfg): softmax over identical
-        # keys is uniform -> cross-attention output = to_out(v_row); see DiT_TriLatent._context_kv
-        rows = _attention_rows(ca[..., :1024])
-        if rows is not None:
-            oc = st["oc"]
-            for l, W in enumerate(P["blocks"]):
-                ops.gemm(ckv[l][:, 0, D:].contiguous(), W["co_w"], W["co_b"], out=oc[l])
-            out.update(rows=rows, oconst=oc)
-        return self._ctx_cache.put((vec0, ca0), out)
-
-    @torch.no_grad()
-    def forward(self, x, timesteps=None, context=None, y=None, get_attr="", **kwargs):
-        """x (B, 12, 32, 32); timesteps (B,) float in [0,1]; context {'vector','crossattn'}."""
-        if get_attr != "":
-            return getattr(self, get_attr)
-        assert isinstance(context, dict)
-        if not x.is_cuda:
-            raise RuntimeError("ln3diff_b200 DiT runs on CUDA only (no CPU fallback)")
-        if self._prep is None:
-            self.prepare()
-        t = timesteps.to(device=x.device, dtype=torch.float32).contiguous()
-        return self._run(x, t, self._context(context))
-
-    @torch.no_grad()
-    def forward_with_cfg(self, x, t, context, cfg_scale):
-        """reference dit_i23d.py:155-168 (cond first, uncond second; returns cat([half, half]))."""
-        eps = self.forward(x, t, context)
-        cond_eps, uncond_eps = torch.split(eps, len(eps) // 2, dim=0)
-        half = uncond_eps + cfg_scale * (cond_eps - uncond_eps)
-        return torch.cat([half, half], dim=0)
+        # the closed form covers identical CLIP tokens (the all-zero unconditional half of forward_with_cfg)
+        return self._ctx_cache.put((vec0, ca0), cross_attention_context(split_kv(ckv), ca[..., :1024], P["blocks"],
+                                                                        st["oc"], cls=cls, dkv=split_kv(dkv)))
 
 
 class DiT_I23D_PixelArt_MVCond_noClip(DiT_I23D_PixelArt):
@@ -228,7 +149,7 @@ class DiT_I23D_PixelArt_MVCond_noClip(DiT_I23D_PixelArt):
     model without dino_proj / clip_spatial_proj / cap_embedder, so t = t_embedder(timesteps) alone, and
     `ImageCondDiTBlockPixelArtRMSNormNoClip` blocks: self-attention over the 768 latent tokens only and
     cross-attention to the flattened multi-view DINO tokens context['concat'] (B, V, 256, C) -> (B, V*256, C), with
-    no attention_y_norm.  Same launch sequence as DiT_I23D_PixelArt (`pixart_forward`): the pooled embedding is a
+    no attention_y_norm.  Same launch sequence as DiT_I23D_PixelArt: the pooled embedding is a
     zero row, there is no second self-attention K/V source, and every layer's cross-attention K|V of the DINO tokens
     is computed once per condition batch."""
     _vit_blk = ImageCondDiTBlockPixelArtRMSNormNoClip
@@ -244,10 +165,10 @@ class DiT_I23D_PixelArt_MVCond_noClip(DiT_I23D_PixelArt):
         del self.dino_proj
         del self.clip_spatial_proj, self.cap_embedder
 
-    def _prepare_context_weights(self, bf, f32) -> dict:
+    def _pack_context(self, bf, f32) -> dict:
         return {}
 
-    def _prepare_block_context_weights(self, b, bf, f32) -> dict:
+    def _pack_dino_block(self, b, bf, f32) -> dict:
         return {}
 
     @torch.no_grad()
@@ -271,15 +192,8 @@ class DiT_I23D_PixelArt_MVCond_noClip(DiT_I23D_PixelArt):
         ckv = st["ckv"]
         for l, W in enumerate(P["blocks"]):
             ops.gemm(ctx, W["ckv_w"], out=ckv[l].view(B * Lc, 2 * D), head_norm=W["ck_norm"], head_norm_sec_cols=D)
-        out = dict(cls=st["cls"], ckv=ckv, rows=(0, B), oconst=None)
-        # the all-zero unconditional half: closed-form cross-attention (see DiT_I23D_PixelArt._context)
-        rows = _attention_rows(tok)
-        if rows is not None:
-            oc = st["oc"]
-            for l, W in enumerate(P["blocks"]):
-                ops.gemm(ckv[l][:, 0, D:].contiguous(), W["co_w"], W["co_b"], out=oc[l])
-            out.update(rows=rows, oconst=oc)
-        return self._ctx_cache.put((ca0,), out)
+        return self._ctx_cache.put((ca0,), cross_attention_context(split_kv(ckv), tok, P["blocks"], st["oc"],
+                                                                   cls=st["cls"]))
 
 
 def _mk(depth, hidden, heads, cls=DiT_I23D_PixelArt):

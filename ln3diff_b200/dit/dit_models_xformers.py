@@ -3,7 +3,7 @@
 The classes below are *parameter containers with the reference's names and state_dict keys*
 (`blocks.{i}.attn.qkv.weight`, `blocks.{i}.mlp.mlp.0.weight`, `blocks.{i}.cross_attn.to_q.weight`,
 `final_layer.adaLN_modulation.1.weight`, ... -- SURVEY.md appendix B) so checkpoints of the
-reference load unchanged.  Their arithmetic runs in `ln3diff_b200.dit.engine` on hand-written
+reference load unchanged.  Their arithmetic runs in `ln3diff_b200.dit._denoiser` on hand-written
 sm_90a kernels; there is no PyTorch-eager fallback.
 """
 from __future__ import annotations

@@ -158,7 +158,7 @@ def test_bench_cross_attention(dev):
 @pytest.mark.parametrize("B,H,Lq,Lkv,Lkv2", [
     (8, 16, 768, 256, 0),       # PixArt cross-attention
     (8, 16, 768, 1536, 0),      # MV23D cross-attention
-    (4, 16, 768, 768, 257),     # self-attention with a second K/V source (_pixart.py)
+    (4, 16, 768, 768, 257),     # self-attention with a second K/V source (dit/_denoiser.py)
     (12, 16, 256, 256, 0),      # DiT2 decoder, in-plane attention (3 B x 256 tokens)
     (4, 16, 768, 768, 0),       # DiT2 decoder, global attention
 ])

@@ -176,7 +176,7 @@ def run_case(dev, M, N, K, *, bias=True, act=0, out_kind=0, ldo=None, gate_rows=
 # ------------------------------------------------------------------ cases
 B, T, D = 16, 768, 1024        # bench.py's DiT-L/2 forward: 8 prompts with CFG, 768 tokens
 
-HOT = {                        # name: (M, N, K, bias, act) of dit_trilatent._forward_impl
+HOT = {                        # name: (M, N, K, bias, act) of _denoiser.run_blocks
     "qkv": (B * T, 3 * D, D, True, 0),
     "proj": (B * T, D, D, True, 0),
     "cross_q": (B * T // 2, D, D, False, 0),

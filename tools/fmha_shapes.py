@@ -29,7 +29,7 @@ from gemm_shapes import ClockPoll, smi, time_window  # noqa: E402
 
 # name, B, H, Lq, Lkv, Lkv2 (second K/V source), causal, layout
 #   packed: q/k/v are column slices of one (B, L, 3 H 64) buffer (dit_trilatent.py:323, vit_triplane.py:209)
-#   kv:     q (B, Lq, H 64) and K/V slices of one (B, Lkv, 2 H 64) buffer (_pixart.py:63)
+#   kv:     q (B, Lq, H 64) and K/V slices of one (B, Lkv, 2 H 64) buffer (dit/_denoiser.py:split_kv)
 #   layers: K/V of one layer inside a (B, Lkv, layers, 2, H 64) cache, the output a sub-batch view of a batch of
 #           2 B (dit_trilatent.py:337)
 SHAPES = [

@@ -2,7 +2,7 @@
 
     python tools/gemm_shapes.py [--lib PATH [--lib PATH ...]] [--rounds R] [--window-s S]
 
-The first six shapes are the per-layer GEMMs of `dit/dit_trilatent.py::_forward_impl` at bench.py's batch (8 prompts
+The first six shapes are the per-layer GEMMs of `dit/_denoiser.py::run_blocks` at bench.py's batch (8 prompts
 with CFG = 16 samples of 768 tokens, D = 1024), each with its production epilogue; fc1 runs the default
 erf-GELU.  The last is the CLIP text tower's qkv for 8 prompts (616 rows, a small GEMM of partial tiles).  The
 yardstick is `torch.nn.functional.linear` in bf16 (cuBLAS), with `F.gelu` applied separately for fc1.  Every entry is timed with CUDA events over enough back-to-back launches to fill a window of
