@@ -338,6 +338,9 @@ typedef struct ln3_render_args {
 } ln3_render_args;
 
 size_t ln3_render_workspace_bytes(int V, int M, int group_size);
+/* The schedule ln3_render_views takes for M rays per view and args->image_w: the image width when the kernel
+ * walks 4x4 pixel tiles, 0 when it walks the rays in plain order (16 consecutive rays per work item). */
+int ln3_render_tile_width(int M, int image_w);
 int ln3_render_views(const ln3_render_args* args, void* stream);
 
 /* ------------------------------------------------------------------ tri-plane point queries

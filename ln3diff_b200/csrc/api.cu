@@ -162,6 +162,10 @@ size_t ln3_render_workspace_bytes(int V, int M, int group_size) {
   if (V <= 0 || M <= 0 || group_size <= 0) return 0;
   return render_workspace_bytes(V, M, group_size);
 }
+int ln3_render_tile_width(int M, int image_w) {
+  if (M <= 0) return 0;
+  return render_tile_width(M, image_w);
+}
 int ln3_render_views(const ln3_render_args* args, void* stream) {
   if (!args) return set_error(LN3_EINVAL, "render: null args");
   return render_views(args, static_cast<cudaStream_t>(stream));

@@ -49,6 +49,12 @@ __global__ void render_init_kernel(int* keys, int G) {
   }
 }
 
+// torch.max / torch.min of two tensors propagate a NaN operand; fmaxf / fminf would drop it.  A ray with an
+// exactly-zero direction component whose origin lies on that slab's face gets t = 0 * inf = NaN: the reference
+// then finds end > start false and treats the ray as invalid (it inherits the group's start range).
+__device__ __forceinline__ float max_nan(float a, float b) { return (a != a) ? a : (b != b) ? b : fmaxf(a, b); }
+__device__ __forceinline__ float min_nan(float a, float b) { return (a != a) ? a : (b != b) ? b : fminf(a, b); }
+
 // math_utils.get_ray_limits_box (math_utils.py:124-190), IEEE op for op.
 __global__ void __launch_bounds__(256)
 ray_limits_kernel(const float* __restrict__ ray_o, const float* __restrict__ ray_d, int V, int M,
@@ -67,13 +73,13 @@ ray_limits_kernel(const float* __restrict__ ray_o, const float* __restrict__ ray
     const float tymin = __fmul_rn(__fsub_rn(n1 ? hi : lo, o1), i1);
     const float tymax = __fmul_rn(__fsub_rn(n1 ? lo : hi, o1), i1);
     if (tmin > tymax || tymin > tmax) valid = false;
-    tmin = fmaxf(tmin, tymin);
-    tmax = fminf(tmax, tymax);
+    tmin = max_nan(tmin, tymin);
+    tmax = min_nan(tmax, tymax);
     const float tzmin = __fmul_rn(__fsub_rn(n2 ? hi : lo, o2), i2);
     const float tzmax = __fmul_rn(__fsub_rn(n2 ? lo : hi, o2), i2);
     if (tmin > tzmax || tzmin > tmax) valid = false;
-    tmin = fmaxf(tmin, tzmin);
-    tmax = fminf(tmax, tzmax);
+    tmin = max_nan(tmin, tzmin);
+    tmax = min_nan(tmax, tzmax);
   }
   if (!valid) {
     tmin = -1.f;
@@ -668,6 +674,11 @@ __global__ void render_finalize_kernel(float* depth, const int* keys, int V, int
   depth[r] = fminf(fmaxf(d, lo), hi);
 }
 
+// 2-D tile schedule when a view is an image whose width and height are multiples of 4, else 0 (linear order)
+int render_tile_width(int M, int image_w) {
+  return (image_w > 0 && image_w % 4 == 0 && M % image_w == 0 && (M / image_w) % 4 == 0) ? image_w : 0;
+}
+
 size_t render_workspace_bytes(int V, int M, int group_size) {
   const int G = (V + group_size - 1) / group_size;
   return static_cast<size_t>(G) * 4 * sizeof(int) + static_cast<size_t>(V) * M * 2 * sizeof(float) + 256;
@@ -709,9 +720,7 @@ int render_views(const ln3_render_args* a, cudaStream_t stream) {
   p.keys = keys;
   p.limits = limits;
   p.V = a->V; p.M = a->M; p.H = a->H; p.W = a->W;
-  // 2-D tile schedule when a view is an image whose width and height are multiples of 4
-  p.image_w = (a->image_w > 0 && a->image_w % 4 == 0 && a->M % a->image_w == 0 && (a->M / a->image_w) % 4 == 0)
-                  ? a->image_w : 0;
+  p.image_w = render_tile_width(a->M, a->image_w);
   p.group_size = a->group_size;
   p.views_per_obj = a->views_per_obj > 0 ? a->views_per_obj : 1;
   p.coord_scale = static_cast<float>(2.0 / a->box_warp);

@@ -451,14 +451,24 @@ def render_views(planes_cl: torch.Tensor, ray_o: torch.Tensor, ray_d: torch.Tens
     a.group_size, a.views_per_obj, a.white_back = group_size, views_per_obj, int(white_back)
     a.box_warp, a.bbox_min, a.bbox_max = box_warp, bbox_min, bbox_max
     a.mlp_precision = _lib.MLP_TF32 if mlp_tf32 else _lib.MLP_FP32
+    a.image_w = _render_image_width(M, image_width)
+    _lib.check(_lib.lib().ln3_render_views(C.byref(a), _lib.current_stream()), "ln3_render_views")
+    return out
+
+
+def _render_image_width(M: int, image_width: int | None) -> int:
     # rays in RaySampler order (m = y*W + x): square views get the 4x4 pixel-tile schedule; image_width=0 forces
     # the plain ray order (rays that are not an image, e.g. PatchRaySampler training patches)
     if image_width is None:
         r = int(round(M ** 0.5))
         image_width = r if r * r == M else 0
-    a.image_w = int(image_width) if os.environ.get("LN3_RENDER_TILES", "1") != "0" else 0
-    _lib.check(_lib.lib().ln3_render_views(C.byref(a), _lib.current_stream()), "ln3_render_views")
-    return out
+    return int(image_width) if os.environ.get("LN3_RENDER_TILES", "1") != "0" else 0
+
+
+def render_tile_width(M: int, image_width: int | None = None) -> int:
+    """The schedule render_views(..., image_width=image_width) takes for M rays per view: the width of the image
+    whose 4x4 pixel tiles the kernel walks, or 0 for the plain ray order (16 consecutive rays per work item)."""
+    return int(_lib.lib().ln3_render_tile_width(M, _render_image_width(M, image_width)))
 
 
 def query_points(planes_cl: torch.Tensor, osg: tuple, *, points: torch.Tensor | None = None,

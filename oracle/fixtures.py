@@ -55,6 +55,39 @@ def render_inputs(res: int, n_views: int = len(RENDER_CAM_ROWS), plane_res: int 
     return planes, (w1, b1, w2, b2), nc, nf
 
 
+def render_group_inputs(res: int = 6):
+    """Three objects, one view each, rendered as ONE reference call (batch 3), with edge rays:
+      view 0  rays from z = 2 that hit the box, except rays 0-4: origins on a box face with the matching direction
+              component +0.0 or -0.0 (t = 0 * inf = NaN: the reference marks them invalid), and ray 2 with zero
+              x / y components strictly inside those slabs (valid)
+      view 1  origins inside the box, two of them axis-aligned
+      view 2  every ray misses: only the call's shared start range and depth clamp give it depths.
+    Returns planes (3,3,32,16,16) (object n for view n), osg, ray_o / ray_d (3,res*res,3), noise (3,res*res,64) x2."""
+    planes0, osg, _, _ = render_inputs(res, n_views=1)
+    g = torch.Generator().manual_seed(51)
+    planes = torch.stack([planes0, 5 * torch.randn(planes0.shape, generator=g),
+                          5 * torch.randn(planes0.shape, generator=g)])
+    M = res * res
+    n = torch.nn.functional.normalize
+    o0 = torch.randn(M, 3, generator=g) * 0.1 + torch.tensor([0.0, 0.0, 2.0])
+    d0 = n(-o0 + 0.05 * torch.randn(M, 3, generator=g), dim=1)
+    edge = [((-0.45, 0.0, 2.0), (0.0, 0.0, -1.0)),     # on the x = lo face, d_x = +0
+            ((0.45, 0.1, 2.0), (-0.0, 0.0, -1.0)),     # on the x = hi face, d_x = -0
+            ((0.1, 0.0, 2.0), (0.0, 0.0, -1.0)),       # d_x = d_y = 0 inside the slabs: valid
+            ((0.2, 0.45, -2.0), (0.0, 0.0, 1.0)),      # on the y = hi face, d_y = +0
+            ((-0.45, -0.45, 2.0), (0.0, -0.0, -1.0))]  # on an edge: two NaN slabs
+    for i, (oo, dd) in enumerate(edge):
+        o0[i], d0[i] = torch.tensor(oo), torch.tensor(dd)
+    o1 = (torch.rand(M, 3, generator=g) - 0.5) * 0.6
+    d1 = n(torch.randn(M, 3, generator=g), dim=1)
+    d1[0], d1[1] = torch.tensor([1.0, 0.0, 0.0]), torch.tensor([0.0, -1.0, 0.0])
+    o2 = torch.tensor([3.0, 3.0, 3.0]) + 0.1 * torch.randn(M, 3, generator=g)
+    d2 = n(torch.tensor([1.0, 0.2, 0.1]) + 0.05 * torch.randn(M, 3, generator=g), dim=1)
+    nc = torch.rand(3, M, 64, generator=g)
+    nf = torch.rand(3, M, 64, generator=g)
+    return planes, osg, torch.stack([o0, o1, o2]), torch.stack([d0, d1, d2]), nc, nf
+
+
 DECODER_ARCH, DECODER_DIM = "DiT2-S/2", 384
 SCALING_DIVIDER = 0.96806  # --triplane_scaling_divider of the release scripts
 

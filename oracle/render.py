@@ -227,6 +227,47 @@ def render_rays(planes, osg, ray_o, ray_d, opts, noise_coarse, noise_fine, retur
     return out
 
 
+def render_group(planes_per_view, osg, ray_o, ray_d, noise_coarse, noise_fine, opts):
+    """One reference call of ImportanceRenderer.forward with batch N: view n samples planes_per_view[n], and
+    the call's two global reductions are taken over all N*M rays -- the invalid-ray start/end fix-up
+    (renderer.py:151-155) and the depth clamp range (ray_marcher.py:59-61).
+    planes_per_view (N,3,C,H,W); ray_o/ray_d (N,M,3); noise_coarse (N,M,S); noise_fine (N,M,S_imp).
+    Runs in the dtype of its inputs (float64 inputs: a float64 reference).
+    Returns dict(rgb (N,M,3), depth (N,M,1), weights (N,M,1), valid (N,M))."""
+    S, S_imp = opts["depth_resolution"], opts["depth_resolution_importance"]
+    N, M, _ = ray_o.shape
+    assert opts["ray_start"] == opts["ray_end"] == "auto"
+    start, end = ray_limits_box(ray_o, ray_d, opts["box_warp"])  # (N,M,1)
+    valid = end > start
+    if bool(valid.any()):
+        smin, smax = start[valid].min(), start[valid].max()
+        start = torch.where(valid, start, smin.expand_as(start))
+        end = torch.where(valid, end, smax.expand_as(end))
+    steps = torch.arange(S, dtype=torch.float32).to(start.dtype) / (S - 1)
+    z_all, rgb_all, sig_all = [], [], []
+    for n in range(N):
+        o, d, s, e = ray_o[n], ray_d[n], start[n], end[n]
+        z_c = s + steps[None, :] * (e - s) + noise_coarse[n] * ((e - s) / (S - 1))
+        pts = o[:, None, :] + z_c[:, :, None] * d[:, None, :]
+        rgb_c, sig_c, _ = run_model(planes_per_view[n], osg, pts.reshape(-1, 3), opts)
+        rgb_c, sig_c = rgb_c.reshape(M, S, 3), sig_c.reshape(M, S, 1)
+        _, _, w_c = ray_march(rgb_c, sig_c, z_c[:, :, None], opts["white_back"])
+        z_f, _ = sample_importance(z_c, w_c[:, :, 0], S_imp, noise_fine[n])
+        pts_f = o[:, None, :] + z_f[:, :, None] * d[:, None, :]
+        rgb_f, sig_f, _ = run_model(planes_per_view[n], osg, pts_f.reshape(-1, 3), opts)
+        z = torch.cat([z_c, z_f], 1)
+        order = torch.sort(z, dim=1, stable=True)[1]
+        z_all.append(torch.gather(z, 1, order))
+        rgb_all.append(torch.gather(torch.cat([rgb_c, rgb_f.reshape(M, S_imp, 3)], 1), 1,
+                                    order[:, :, None].expand(-1, -1, 3)))
+        sig_all.append(torch.gather(torch.cat([sig_c, sig_f.reshape(M, S_imp, 1)], 1), 1, order[:, :, None]))
+    # one march over all N*M rays: its depth clamp takes min / max of every view's sorted depths
+    rgb, depth, w = ray_march(torch.cat(rgb_all), torch.cat(sig_all), torch.cat(z_all)[:, :, None],
+                              opts["white_back"])
+    return dict(rgb=rgb.reshape(N, M, 3), depth=depth.reshape(N, M, 1), weights=w.sum(1).reshape(N, M, 1),
+                valid=valid[..., 0])
+
+
 def render_view(planes, osg, cam: torch.Tensor, res: int, opts, noise_coarse, noise_fine):
     """Triplane.forward for one camera row (25,): returns image_raw (3,res,res), image_depth
     (1,res,res), weights_samples (1,res,res), image_mask (1,res,res)."""

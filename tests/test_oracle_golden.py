@@ -89,6 +89,24 @@ def test_render_edge_cases():
     assert bool(r2["valid"].all()) and torch.isfinite(r2["rgb"]).all()
 
 
+def test_render_group_matches_reference(golden):
+    """oracle.render.render_group vs one batch-3 ImportanceRenderer.forward call (render_group.npz): shared start
+    range and depth clamp across the views, NaN slab tests (origin on a face, zero direction component) invalid."""
+    g = golden("render_group.npz")
+    planes, osg, o, d, nc, nf = fx.render_group_inputs()
+    assert torch.equal(o, torch.from_numpy(g["ray_o"])) and torch.equal(d, torch.from_numpy(g["ray_d"]))
+    r = orender.render_group(planes, osg, o, d, nc, nf, orender.OBJAVERSE_OPTS)
+    for k in ("rgb", "depth", "weights"):
+        assert (r[k] - torch.from_numpy(g[k])).abs().max() < 2e-6, k    # fp32 vs fp32, summation order only
+    assert r["valid"][0, :5].tolist() == [False, False, True, False, False]
+    assert bool(r["valid"][1].all()) and not bool(r["valid"][2].any())
+    # the fixture tells one batched call from three per-view calls: the NaN rays of view 0 march the shared
+    # start range, and the all-miss view's depth is clamped to the shared range
+    for v, k in ((0, "rgb"), (2, "depth")):
+        one = orender.render_rays(planes[v], osg, o[v], d[v], orender.OBJAVERSE_OPTS, nc[v], nf[v])
+        assert (one[k] - torch.from_numpy(g[k][v])).abs().max() > 1e-2, (v, k)
+
+
 def test_vae_decoder_matches_reference(golden):
     from oracle import decoder as odec
     from ln3diff_b200.utils import build_ae_decoder
