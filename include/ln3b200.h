@@ -446,15 +446,25 @@ int ln3_pack_frames(const ln3_pack_frames_args* args, void* stream);
  *   f = identity, or the fused GroupNorm-apply (+ swish): v*in_scale[n,c] + in_shift[n,c]
  *       (model.py:46-52 nonlinearity / Normalize; scale/shift from ln3_groupnorm_stats)
  *   up = identity or nearest 2x (Upsample, model.py:54-69): x is then [N, H/2, W/2, Cin]
- *   w is the Conv2d weight repacked to [ksize*ksize, Cin, Cout].
+ *   w is the Conv2d weight repacked to [ksize*ksize, Cin, Cout].  H, W are the OUTPUT dims.
+ *   LN3_EUNSUPPORTED for ksize not 1 or 3.  LN3_EINVAL for a precision other than LN3_MLP_FP32 / LN3_MLP_TF32
+ *   (TF32 applies to ksize 3; ksize 1 always runs fp32), N < 0, non-positive H, W, Cin or Cout, upsample with odd
+ *   H or W, only one of in_scale / in_shift, or a NULL x, w or out -- checked before N == 0 returns without a launch.
+ * ln3_conv_cout_tile: the output channels per CTA (32 or 64) ln3_conv_nhwc takes for these dims: 32 when
+ *   Cout < 64 or when 64-channel CTAs would give fewer than two per SM of the current device (64 regardless of
+ *   the SM count when the environment sets LN3_CONV_COT64=1, read once per process); 0 for a non-positive argument.
  * ln3_groupnorm_stats: torch.nn.GroupNorm(G, C, eps) statistics of x [N, HW, C] folded with the
- *   affine parameters into per-(image, channel) scale / shift [N, C].
+ *   affine parameters into per-(image, channel) scale / shift [N, C].  N <= 0 returns without a launch;
+ *   otherwise LN3_EINVAL for non-positive G, C or HW, C % G != 0, C / G > 256 or a NULL pointer.
  * ln3_attn_single_head: MemoryEfficientAttnBlock core (model.py:209-272): softmax(q k^T/sqrt(C)) v,
- *   q/k/v/out fp32 [N, L, C], one head of width C (128 in conv_sr).
+ *   q/k/v/out fp32 [N, L, C], one head of width C (128 in conv_sr).  N <= 0 returns without a launch;
+ *   otherwise LN3_EINVAL for L <= 0 or a NULL pointer, LN3_EUNSUPPORTED for C not 32, 64 or 128.
  * ln3_patch_embed_triplane: Conv2d(3*Cz -> 3*E, k=s=2, groups=3) + the reference's
  *   (B,3E,h,w)->(B,E,3,h,w)->(B,3hw,E) reshape; x fp32 [B, 3*Cz, S, S] is pre-multiplied by in_mul
  *   (triplane_scaling_divider, nsr/train_util_diffusion.py:188); optional bf16 SiLU copy of the
- *   tokens (the adaLN operand of every DiT2 block, dit/dit_decoder.py:29-31).
+ *   tokens (the adaLN operand of every DiT2 block, dit/dit_decoder.py:29-31).  B <= 0 returns without a
+ *   launch; otherwise LN3_EINVAL for Cz outside 1..16, odd or non-positive S, E <= 0 or a NULL x, w or tokens
+ *   (bias and silu_bf16 may be NULL).
  */
 typedef struct ln3_conv_args {
   const float* x;
@@ -469,6 +479,7 @@ typedef struct ln3_conv_args {
 } ln3_conv_args;
 
 int ln3_conv_nhwc(const ln3_conv_args* args, void* stream);
+int ln3_conv_cout_tile(int N, int H, int W, int Cout);
 int ln3_groupnorm_stats(const float* x, const float* gamma, const float* beta, int N, int HW, int C,
                         int G, float eps, float* scale, float* shift, void* stream);
 int ln3_attn_single_head(const float* q, const float* k, const float* v, float* out, int N, int L,

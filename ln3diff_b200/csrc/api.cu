@@ -198,6 +198,10 @@ int ln3_pack_frames(const ln3_pack_frames_args* args, void* stream) {
   return pack_frames(args, static_cast<cudaStream_t>(stream));
 }
 
+int ln3_conv_cout_tile(int N, int H, int W, int Cout) {
+  if (N <= 0 || H <= 0 || W <= 0 || Cout <= 0) return 0;
+  return conv_cout_tile(N, H, W, Cout);
+}
 int ln3_conv_nhwc(const ln3_conv_args* args, void* stream) {
   if (!args) return set_error(LN3_EINVAL, "conv: null args");
   return conv_nhwc(args, static_cast<cudaStream_t>(stream));

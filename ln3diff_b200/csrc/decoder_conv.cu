@@ -220,20 +220,31 @@ conv3x3_tf32_kernel(const ln3_conv_args a) {
   }
 }
 
+// 64 output channels per CTA, or 32 when the 64-channel grid would leave the GPU under two CTAs per SM (the 16 x 16
+// and 32 x 32 levels of the VAE decoder: 192 CTAs; the kernel is bound by the latency of its staging loads -- ncu
+// long_scoreboard 8.5 cycles per issue, 16 % warps active -- so more, smaller CTAs hide more of it).  LN3_CONV_COT64=1
+// (read once) keeps 64 whenever Cout >= 64.
+int conv_cout_tile(int N, int H, int W, int Cout) {
+  static const bool cot_auto = !(getenv("LN3_CONV_COT64") && atoi(getenv("LN3_CONV_COT64")) != 0);
+  if (Cout < 64) return 32;
+  const long long tiles = static_cast<long long>((H + kCT - 1) / kCT) * ((W + kCT - 1) / kCT);
+  if (cot_auto && tiles * ((Cout + 63) / 64) * N < 2LL * device_sm_count()) return 32;
+  return 64;
+}
+
 int conv_nhwc(const ln3_conv_args* a, cudaStream_t stream) {
-  if (a->N <= 0) return LN3_OK;
   if (a->ksize != 1 && a->ksize != 3) return set_error(LN3_EUNSUPPORTED, "conv: ksize must be 1 or 3");
+  if (a->precision != LN3_MLP_FP32 && a->precision != LN3_MLP_TF32)
+    return set_error(LN3_EINVAL, "conv: precision must be LN3_MLP_FP32 or LN3_MLP_TF32");
+  if (a->N < 0 || a->H <= 0 || a->W <= 0 || a->Cin <= 0 || a->Cout <= 0)
+    return set_error(LN3_EINVAL, "conv: need N >= 0 and positive H, W, Cin, Cout");
   if (a->upsample && ((a->H | a->W) & 1)) return set_error(LN3_EINVAL, "conv: upsample needs even H, W");
   if ((a->in_scale == nullptr) != (a->in_shift == nullptr))
     return set_error(LN3_EINVAL, "conv: in_scale / in_shift must be given together");
   if (!a->x || !a->w || !a->out) return set_error(LN3_EINVAL, "conv: null pointer");
+  if (a->N == 0) return LN3_OK;
   const int tiles = ((a->H + kCT - 1) / kCT) * ((a->W + kCT - 1) / kCT);
-  // 64 output channels per CTA, or 32 when the 64-channel grid would leave the GPU under two CTAs per SM (the 16 x 16
-  // and 32 x 32 levels of the VAE decoder: 192 CTAs; the kernel is bound by the latency of its staging loads --
-  // ncu long_scoreboard 8.5 cycles per issue, 16 % warps active -- so more, smaller CTAs hide more of it)
-  static const bool cot_auto = !(getenv("LN3_CONV_COT64") && atoi(getenv("LN3_CONV_COT64")) != 0);
-  int cot = (a->Cout >= 64) ? 64 : 32;
-  if (cot == 64 && cot_auto && static_cast<long long>(tiles) * ((a->Cout + 63) / 64) * a->N < 2 * device_sm_count()) cot = 32;
+  const int cot = conv_cout_tile(a->N, a->H, a->W, a->Cout);
   dim3 grid(tiles, (a->Cout + cot - 1) / cot, a->N);
   if (a->ksize == 3 && a->precision == LN3_MLP_TF32) {
     if (cot == 64) conv3x3_tf32_kernel<64, false><<<grid, 256, 0, stream>>>(*a);
@@ -382,6 +393,7 @@ groupnorm_stats_kernel(const float* __restrict__ x, const float* __restrict__ ga
 int groupnorm_stats(const float* x, const float* gamma, const float* beta, int N, int HW, int C, int G,
                     float eps, float* scale, float* shift, cudaStream_t stream) {
   if (N <= 0) return LN3_OK;
+  if (G <= 0 || C <= 0 || HW <= 0) return set_error(LN3_EINVAL, "groupnorm: need positive G, C, HW");
   if (C % G != 0 || C / G > 256) return set_error(LN3_EINVAL, "groupnorm: bad C / G");
   groupnorm_stats_kernel<<<dim3(G, N), 256, 0, stream>>>(x, gamma, beta, HW, C, G, eps, scale, shift);
   cudaError_t e = cudaGetLastError();
@@ -470,6 +482,7 @@ attn_single_head_kernel(const float* __restrict__ q, const float* __restrict__ k
 int attn_single_head(const float* q, const float* k, const float* v, float* out, int N, int L, int C,
                      cudaStream_t stream) {
   if (N <= 0) return LN3_OK;
+  if (L <= 0) return set_error(LN3_EINVAL, "attn_single_head: need L > 0");
   const dim3 grid((L + 7) / 8, N);
   const float scale = 1.0f / sqrtf(static_cast<float>(C));
   switch (C) {
@@ -521,6 +534,7 @@ int patch_embed_triplane(const float* x, const float* w, const float* bias, int 
                          float in_mul, float* tokens, void* silu_bf16, cudaStream_t stream) {
   if (B <= 0) return LN3_OK;
   if (Cz <= 0 || Cz > 16 || (S & 1)) return set_error(LN3_EINVAL, "patch_embed_triplane: need 1 <= Cz <= 16, even S");
+  if (S <= 0 || E <= 0) return set_error(LN3_EINVAL, "patch_embed_triplane: need positive S, E");
   const int L = (S / 2) * (S / 2);
   patch_embed_triplane_kernel<<<B * 3 * L, 256, 0, stream>>>(x, w, bias, B, Cz, S, E, in_mul, tokens,
                                                              reinterpret_cast<__nv_bfloat16*>(silu_bf16));

@@ -87,6 +87,7 @@ size_t marching_cubes_workspace_bytes(int nx, int ny, int nz);
 int marching_cubes_count(const ln3_marching_cubes_args* a, cudaStream_t stream);
 int marching_cubes_emit(const ln3_marching_cubes_args* a, cudaStream_t stream);
 
+int conv_cout_tile(int N, int H, int W, int Cout);
 int conv_nhwc(const ln3_conv_args* a, cudaStream_t stream);
 int groupnorm_stats(const float* x, const float* gamma, const float* beta, int N, int HW, int C, int G,
                     float eps, float* scale, float* shift, cudaStream_t stream);

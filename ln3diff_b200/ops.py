@@ -547,6 +547,11 @@ def conv_nhwc(x: torch.Tensor, w_packed: torch.Tensor, bias: torch.Tensor | None
     return out
 
 
+def conv_cout_tile(N: int, H: int, W: int, Cout: int) -> int:
+    """The output channels per CTA (32 or 64) conv_nhwc takes for an (N, H, W, Cout) output on the current device."""
+    return int(_lib.lib().ln3_conv_cout_tile(N, H, W, Cout))
+
+
 def downsample_nhwc(x: torch.Tensor, w_packed: torch.Tensor, bias: torch.Tensor | None, *,
                     out: torch.Tensor | None = None, tf32: bool = False) -> torch.Tensor:
     """The encoder's Downsample: 3x3 conv, stride 2, on F.pad(x, (0,1,0,1)).  x (N,H,W,Cin) NHWC fp32 with H, W

@@ -217,10 +217,19 @@ class RodinSR_256_fusionv6_ConvQuant_liteSR_dinoInit3DAttn_SD_B_3L_C_withrollout
             ops.gemm(hbuf, W["fc2_w"], W["fc2_b"], out=val)
         ops.norm_modulate(x2, norm=NORM_LAYER, resid=val, resid_gate=mod[:, 5 * D:6 * D], resid_gate_rows=1, want_out=False)
         # tokens (B, 3*16*16, D) are already NHWC (3B, 16, 16, D)
-        S = P["sr"]
         ts = self.token_size
+        out = self._conv_sr(x.view(B * 3, ts, ts, D))
+        return out.view(B, 3, out.shape[1], out.shape[2], out.shape[3])
+
+    @torch.no_grad()
+    def _conv_sr(self, h):
+        """superresolution['conv_sr'] (the ldm Decoder) on NHWC fp32 tokens (3B, 16, 16, D) -> the channels-last
+        planes (3B, 128, 128, 32)."""
+        if self._prep is None:
+            self.prepare()
+        S = self._prep["sr"]
         tf = self.conv_tf32
-        h = ops.conv_nhwc(x.view(B * 3, ts, ts, D), *S["conv_in"], ksize=3, tf32=tf)
+        h = ops.conv_nhwc(h, *S["conv_in"], ksize=3, tf32=tf)
         h = self._res(h, S["mid1"])
         A = S["attn"]
         gn = ops.groupnorm_stats(h, *A["n"])
@@ -232,8 +241,7 @@ class RodinSR_256_fusionv6_ConvQuant_liteSR_dinoInit3DAttn_SD_B_3L_C_withrollout
                 h = self._res(h, W)
             if S["up"][lvl]["upsample"] is not None:
                 h = ops.conv_nhwc(h, *S["up"][lvl]["upsample"], ksize=3, upsample=True, tf32=tf)
-        out = ops.conv_nhwc(h, *S["conv_out"], ksize=3, gn=ops.groupnorm_stats(h, *S["nout"]), swish=True, tf32=tf)
-        return out.view(B, 3, out.shape[1], out.shape[2], out.shape[3])
+        return ops.conv_nhwc(h, *S["conv_out"], ksize=3, gn=ops.groupnorm_stats(h, *S["nout"]), swish=True, tf32=tf)
 
     # ------------------------------------------------------------------ VAE posterior (encoder side)
     @torch.no_grad()

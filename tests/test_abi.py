@@ -40,7 +40,8 @@ def test_ctypes_structs_match_header_field_order():
              "ln3_norm_modulate_args": _lib.NormModulateArgs, "ln3_patch_embed_args": _lib.PatchEmbedArgs,
              "ln3_final_layer_args": _lib.FinalLayerArgs, "ln3_sampler_update_args": _lib.SamplerUpdateArgs,
              "ln3_render_args": _lib.RenderArgs, "ln3_query_points_args": _lib.QueryPointsArgs,
-             "ln3_pack_frames_args": _lib.PackFramesArgs, "ln3_marching_cubes_args": _lib.MarchingCubesArgs}
+             "ln3_pack_frames_args": _lib.PackFramesArgs, "ln3_marching_cubes_args": _lib.MarchingCubesArgs,
+             "ln3_conv_args": _lib.ConvArgs}
     for cname, cls in pairs.items():
         body = re.search(r"typedef struct " + cname + r"\s*\{(.*?)\}\s*" + cname + ";", src, flags=re.S).group(1)
         names = []
