@@ -283,6 +283,71 @@ typedef struct ln3_sampler_update_args {
 
 int ln3_sampler_affine_update(const ln3_sampler_update_args* args, void* stream);
 
+/* ------------------------------------------------------------------ grouped adaptive dopri5
+ * The per-attempt arithmetic of the adaptive Dormand-Prince 5(4) solver that `sample_ode`'s default runs
+ * (transport/transport.py:374-421 -> transport/integrators.py:101-120 -> torchdiffeq odeint(method='dopri5')),
+ * restated in transport/dopri5.py, for G independent problems in one batch.  Row r of the fp32 state
+ * [B, n_per_sample] belongs to group row_group[r]; each group has its own error norm, step size, accept / reject,
+ * counters and end, held in the caller-owned device array `state` [G] of ln3_ode_group.  Times and steps are
+ * float64, as the host solver keeps them; the forward's per-row time is fp32.  No host synchronisation: the caller
+ * reads `status` back (asynchronously) to learn when every group has finished.
+ *   ln3_ode_stage(stage 1..6): y_stage = y + sum_j beta[stage-1][j] * dt_g * k_j (k_0 = f0, k_j = k[j-1]) and
+ *       t_rows[r] = fp32(t_g + alpha[stage-1] * dt_g); stage 0 is the initial-step probe y_stage = y + h0_g * f0,
+ *       t_rows = t_g + h0_g.  Rows of groups whose status is not LN3_ODE_RUNNING are not written.
+ *   ln3_ode_initial_step(phase 0): per group d0 = rms(y / s), d1 = rms(f0 / s), s = atol + rtol |y|, h0 (dt = h0);
+ *       (phase 1, after one forward of the stage-0 probe into k[0]): d2 = rms((k[0] - f0) / s) / h0, h1 and
+ *       dt = min(100 h0, h1) (order 4, Hairer-Norsett-Wanner II.4); nfe = 2.
+ *   ln3_ode_step: after the six stage forwards (k[0..5]; y_stage holds the 5th-order solution y1):
+ *       ratio = rms(err / (atol + rtol max(|y|, |y1|))), err = dt * sum_j c_err[j] k_j; accept iff ratio <= 1;
+ *       dt' = dt * min(ifactor, max(safety / ratio^(1/5), accepted ? 1 : dfactor)), dt * ifactor when ratio == 0;
+ *       on accept y <- y1, f0 <- k[5] (FSAL), and when t reaches t_end the quartic dense output at t_end is written
+ *       to out and the group is done.  Then the checks of the next attempt: accepted + rejected >= max_num_steps
+ *       gives LN3_ODE_EMAXSTEPS, t + dt == t gives LN3_ODE_EUNDERFLOW (the group is frozen; the kernels never trap).
+ * Reductions are deterministic: every row is cut into fixed chunks of 1024 elements whose squares are summed in a
+ * fixed order into `workspace` (float64), and each group sums its rows' partials in row, then chunk, order -- a
+ * group's result does not depend on the other groups in the batch.
+ * LN3_EINVAL unless B, G > 0, n_per_sample > 0 and % 4 == 0, every row_group_host entry in [0, G) with every group
+ * non-empty, workspace_bytes >= ln3_ode_workspace_bytes(B, n_per_sample), the state, row map, time and the buffers
+ * an entry point reads or writes non-NULL, and y, f0, k[], y_stage and out 16-byte aligned.
+ */
+enum { LN3_ODE_RUNNING = 0, LN3_ODE_DONE = 1, LN3_ODE_EMAXSTEPS = -1, LN3_ODE_EUNDERFLOW = -2 };
+
+typedef struct ln3_ode_group {
+  double t;        /* time reached (end of the last accepted step) */
+  double dt;       /* size of the next attempt (h0 between the two initial-step phases) */
+  double t_prev;   /* start of the last accepted step */
+  double dt_step;  /* size of the last attempt */
+  double ratio;    /* error ratio of the last attempt */
+  double aux;      /* initial-step scratch (d1) */
+  int nfe, accepted, rejected;
+  int status;      /* LN3_ODE_RUNNING, LN3_ODE_DONE or a negative LN3_ODE_E* code */
+  int event;       /* last attempt: 0 rejected / not run, 1 accepted, 2 accepted and reached t_end */
+  int reserved;
+} ln3_ode_group;
+
+typedef struct ln3_ode_args {
+  float* y;                     /* [B, n] state, committed on accept */
+  float* f0;                    /* [B, n] derivative at y (FSAL) */
+  const float* k[6];            /* [B, n] stage derivatives of the current attempt */
+  float* y_stage;               /* [B, n] forward input written by ln3_ode_stage */
+  float* t_rows;                /* [B] fp32 forward time written by ln3_ode_stage */
+  float* out;                   /* [B, n] dense output at t_end, written once per group */
+  const int* row_group;         /* device int32 [B] */
+  const int* row_group_host;    /* host copy of row_group, validated on every call */
+  ln3_ode_group* state;         /* device [G] */
+  void* workspace;              /* device, ln3_ode_workspace_bytes(B, n_per_sample) */
+  size_t workspace_bytes;
+  int B, G;
+  long long n_per_sample;
+  double t_end, rtol, atol, safety, ifactor, dfactor;
+  int max_num_steps;
+} ln3_ode_args;
+
+size_t ln3_ode_workspace_bytes(int B, long long n_per_sample);
+int ln3_ode_stage(const ln3_ode_args* args, int stage, void* stream);
+int ln3_ode_initial_step(const ln3_ode_args* args, int phase, void* stream);
+int ln3_ode_step(const ln3_ode_args* args, void* stream);
+
 /* ------------------------------------------------------------------ tri-plane volumetric renderer
  * ln3_render_views: the whole of ImportanceRenderer.forward (nsr/volumetric_rendering/renderer.py:
  * 133-307) for the Objaverse preset (nsr/script_util.py:761-797): 'auto' ray limits against the

@@ -160,6 +160,29 @@ class VaePosteriorArgs(C.Structure):
     ]
 
 
+class OdeGroup(C.Structure):
+    _fields_ = [
+        ("t", C.c_double), ("dt", C.c_double), ("t_prev", C.c_double), ("dt_step", C.c_double),
+        ("ratio", C.c_double), ("aux", C.c_double),
+        ("nfe", C.c_int), ("accepted", C.c_int), ("rejected", C.c_int),
+        ("status", C.c_int), ("event", C.c_int), ("reserved", C.c_int),
+    ]
+
+
+class OdeArgs(C.Structure):
+    _fields_ = [
+        ("y", C.c_void_p), ("f0", C.c_void_p), ("k", C.c_void_p * 6), ("y_stage", C.c_void_p),
+        ("t_rows", C.c_void_p), ("out", C.c_void_p), ("row_group", C.c_void_p), ("row_group_host", C.c_void_p),
+        ("state", C.c_void_p), ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t),
+        ("B", C.c_int), ("G", C.c_int), ("n_per_sample", C.c_longlong),
+        ("t_end", C.c_double), ("rtol", C.c_double), ("atol", C.c_double), ("safety", C.c_double),
+        ("ifactor", C.c_double), ("dfactor", C.c_double),
+        ("max_num_steps", C.c_int),
+    ]
+
+
+ODE_RUNNING, ODE_DONE, ODE_EMAXSTEPS, ODE_EUNDERFLOW = 0, 1, -1, -2
+
 NORM_NONE, NORM_LAYER, NORM_RMS = 0, 1, 2
 MLP_FP32, MLP_TF32 = 0, 1
 
@@ -180,6 +203,8 @@ def lib() -> C.CDLL:
         L.ln3_render_workspace_bytes.restype = C.c_size_t
         L.ln3_gemm_workspace_bytes.restype = C.c_size_t
         L.ln3_marching_cubes_workspace_bytes.restype = C.c_size_t
+        L.ln3_ode_workspace_bytes.restype = C.c_size_t
+        L.ln3_ode_workspace_bytes.argtypes = [C.c_int, C.c_longlong]
         _lib = L
     return _lib
 

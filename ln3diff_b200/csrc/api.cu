@@ -5,6 +5,7 @@
 #include <cstring>
 
 #include <cstdlib>
+#include <vector>
 
 #include "ln3_internal.h"
 
@@ -109,6 +110,42 @@ int make_tmap_3d_bf16(CUtensorMap* out, const void* ptr, long long d0, long long
   if (r != CUDA_SUCCESS)
     return set_error(LN3_ECUDA, "cuTensorMapEncodeTiled(3d %lldx%lldx%lld) -> %d", d2, d1, d0,
                      static_cast<int>(r));
+  return LN3_OK;
+}
+
+// Checks shared by the ln3_ode_* entry points (see include/ln3b200.h); `need` selects the buffers the call reads.
+enum { ODE_NEED_STAGE = 1, ODE_NEED_K = 2, ODE_NEED_K0 = 4, ODE_NEED_OUT = 8, ODE_NEED_WS = 16 };
+
+static bool misaligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) != 0; }
+
+static int ode_validate(const ln3_ode_args* a, int need, const char* what) {
+  if (!a) return set_error(LN3_EINVAL, "%s: null args", what);
+  if (a->B <= 0 || a->G <= 0) return set_error(LN3_EINVAL, "%s: B and G must be positive", what);
+  if (a->n_per_sample <= 0 || a->n_per_sample % 4)
+    return set_error(LN3_EINVAL, "%s: n_per_sample must be a positive multiple of 4", what);
+  if (a->max_num_steps < 0) return set_error(LN3_EINVAL, "%s: max_num_steps < 0", what);
+  if (!a->y || !a->f0 || !a->state || !a->row_group || !a->row_group_host)
+    return set_error(LN3_EINVAL, "%s: null y, f0, state or row map", what);
+  if (misaligned16(a->y) || misaligned16(a->f0))
+    return set_error(LN3_EINVAL, "%s: y and f0 must be 16-byte aligned", what);
+  if ((need & ODE_NEED_STAGE) && (!a->y_stage || !a->t_rows || misaligned16(a->y_stage)))
+    return set_error(LN3_EINVAL, "%s: y_stage (16-byte aligned) and t_rows are required", what);
+  const int nk = (need & ODE_NEED_K) ? 6 : (need & ODE_NEED_K0) ? 1 : 0;
+  for (int j = 0; j < nk; ++j)
+    if (!a->k[j] || misaligned16(a->k[j]))
+      return set_error(LN3_EINVAL, "%s: k[%d] is null or not 16-byte aligned", what, j);
+  if ((need & ODE_NEED_OUT) && (!a->out || misaligned16(a->out)))
+    return set_error(LN3_EINVAL, "%s: out is null or not 16-byte aligned", what);
+  if ((need & ODE_NEED_WS) && (!a->workspace || a->workspace_bytes < ode_workspace_bytes(a->B, a->n_per_sample)))
+    return set_error(LN3_EINVAL, "%s: workspace smaller than ln3_ode_workspace_bytes(B, n_per_sample)", what);
+  std::vector<int> rows(static_cast<size_t>(a->G), 0);
+  for (int r = 0; r < a->B; ++r) {
+    const int g = a->row_group_host[r];
+    if (g < 0 || g >= a->G) return set_error(LN3_EINVAL, "%s: row_group[%d] = %d is outside [0, %d)", what, r, g, a->G);
+    ++rows[g];
+  }
+  for (int g = 0; g < a->G; ++g)
+    if (rows[g] == 0) return set_error(LN3_EINVAL, "%s: group %d has no rows", what, g);
   return LN3_OK;
 }
 
@@ -230,6 +267,31 @@ int ln3_downsample_nhwc(const ln3_conv_args* args, void* stream) {
 int ln3_vae_posterior(const ln3_vae_posterior_args* args, void* stream) {
   if (!args) return set_error(LN3_EINVAL, "vae_posterior: null args");
   return vae_posterior(args, static_cast<cudaStream_t>(stream));
+}
+
+size_t ln3_ode_workspace_bytes(int B, long long n_per_sample) {
+  if (B <= 0 || n_per_sample <= 0) return 0;
+  return ode_workspace_bytes(B, n_per_sample);
+}
+int ln3_ode_stage(const ln3_ode_args* args, int stage, void* stream) {
+  if (stage < 0 || stage > 6) return set_error(LN3_EINVAL, "ode_stage: stage %d is outside 0..6", stage);
+  int rc = ode_validate(args, ODE_NEED_STAGE, "ode_stage");
+  if (rc != LN3_OK) return rc;
+  for (int j = 0; j + 1 < stage; ++j)   // stage i reads k[0 .. i-2]
+    if (!args->k[j] || misaligned16(args->k[j]))
+      return set_error(LN3_EINVAL, "ode_stage: k[%d] is null or not 16-byte aligned", j);
+  return ode_stage(args, stage, static_cast<cudaStream_t>(stream));
+}
+int ln3_ode_initial_step(const ln3_ode_args* args, int phase, void* stream) {
+  if (phase != 0 && phase != 1) return set_error(LN3_EINVAL, "ode_initial_step: phase must be 0 or 1");
+  int rc = ode_validate(args, ODE_NEED_WS | (phase == 1 ? ODE_NEED_K0 : 0), "ode_initial_step");
+  if (rc != LN3_OK) return rc;
+  return ode_initial_step(args, phase, static_cast<cudaStream_t>(stream));
+}
+int ln3_ode_step(const ln3_ode_args* args, void* stream) {
+  int rc = ode_validate(args, ODE_NEED_STAGE | ODE_NEED_K | ODE_NEED_OUT | ODE_NEED_WS, "ode_step");
+  if (rc != LN3_OK) return rc;
+  return ode_step(args, static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

@@ -338,6 +338,106 @@ def sampler_affine_update(x: torch.Tensor, coef: torch.Tensor, m0: torch.Tensor,
     return out
 
 
+# ---------------------------------------------------------------------------------------------- grouped dopri5
+ODE_GROUP_BYTES = C.sizeof(_lib.OdeGroup)
+_ODE_F64 = ("t", "dt", "t_prev", "dt_step", "ratio", "aux")
+_ODE_I32 = ("nfe", "accepted", "rejected", "status", "event")
+
+
+def ode_state(n_groups: int, t0: float, device) -> torch.Tensor:
+    """A fresh per-group state block (uint8 (G, sizeof(ln3_ode_group))) on `device`: t = t_prev = t0, running."""
+    _req(n_groups > 0, "n_groups must be positive")
+    st = torch.zeros(n_groups, ODE_GROUP_BYTES, dtype=torch.uint8)
+    f = st.view(torch.float64)
+    f[:, 0] = t0
+    f[:, 2] = t0
+    return st.to(device)
+
+
+def ode_state_fields(state: torch.Tensor) -> dict:
+    """The fields of a state block (device or host copy) as CPU tensors: float64 t ... aux, int32 nfe ... event."""
+    st = state.detach().cpu().contiguous()
+    f, i = st.view(torch.float64), st.view(torch.int32)
+    out = {k: f[:, j].clone() for j, k in enumerate(_ODE_F64)}
+    out.update({k: i[:, 12 + j].clone() for j, k in enumerate(_ODE_I32)})
+    return out
+
+
+def _ode_buf(t_: torch.Tensor, nm: str, B: int, n: int) -> None:
+    _cuda(t_, nm, torch.float32)
+    _req(t_.is_contiguous() and t_.dim() >= 1 and t_.shape[0] == B and t_.numel() == B * n,
+         f"{nm} must be contiguous with the state's shape")
+    _req(t_.data_ptr() % 16 == 0, f"{nm} must be 16-byte aligned (the kernels use 128-bit accesses)")
+
+
+def ode_args(y: torch.Tensor, f0: torch.Tensor, y_stage: torch.Tensor, t_rows: torch.Tensor, out: torch.Tensor,
+             row_group: torch.Tensor, state: torch.Tensor, *, t_end: float, rtol: float, atol: float,
+             safety: float = 0.9, ifactor: float = 10.0, dfactor: float = 0.2,
+             max_num_steps: int = 2 ** 31 - 1) -> _lib.OdeArgs:
+    """The argument block of the ln3_ode_* entry points.  y, f0, y_stage, out: contiguous fp32 (B, ...) CUDA tensors;
+    t_rows fp32 (B,); row_group int32 (B,) group of each row (any device: a host and a device copy are kept);
+    state from `ode_state`.  The returned struct holds references to every tensor it points to."""
+    _cuda(y, "y", torch.float32)
+    B = y.shape[0]
+    n = y.numel() // max(B, 1)
+    _req(B > 0 and n > 0 and n % 4 == 0, "elements per row must be a positive multiple of 4")
+    for nm, t_ in (("y", y), ("f0", f0), ("y_stage", y_stage), ("out", out)):
+        _ode_buf(t_, nm, B, n)
+    _cuda(t_rows, "t_rows", torch.float32)
+    _req(t_rows.shape == (B,) and t_rows.is_contiguous(), "t_rows must be contiguous (B,)")
+    _req(row_group.dim() == 1 and row_group.shape[0] == B, "row_group must be (B,)")
+    rg_host = row_group.detach().to("cpu", torch.int32).contiguous()
+    G = state.shape[0] if state.dim() == 2 else 0
+    _cuda(state, "state", torch.uint8)
+    _req(state.shape == (G, ODE_GROUP_BYTES) and state.is_contiguous() and state.data_ptr() % 8 == 0,
+         "state must be an ode_state block")
+    rg_dev = rg_host.to(y.device)
+    ws = torch.empty(int(_lib.lib().ln3_ode_workspace_bytes(B, n)), dtype=torch.uint8, device=y.device)
+    a = _lib.OdeArgs()
+    a.y, a.f0, a.y_stage, a.t_rows, a.out = (t_.data_ptr() for t_ in (y, f0, y_stage, t_rows, out))
+    a.row_group, a.row_group_host, a.state = rg_dev.data_ptr(), rg_host.data_ptr(), state.data_ptr()
+    a.workspace, a.workspace_bytes = ws.data_ptr(), ws.numel()
+    a.B, a.G, a.n_per_sample = B, G, n
+    a.t_end, a.rtol, a.atol, a.safety, a.ifactor, a.dfactor = t_end, rtol, atol, safety, ifactor, dfactor
+    a.max_num_steps = max_num_steps
+    a.tensors = (y, f0, y_stage, t_rows, out, rg_dev, rg_host, state, ws)
+    return a
+
+
+def _ode_k(a: _lib.OdeArgs, ks) -> None:
+    _req(len(ks) <= 6, "at most six stage derivatives")
+    for i in range(6):
+        if i < len(ks):
+            _ode_buf(ks[i], f"k[{i}]", a.B, a.n_per_sample)
+            _req(ks[i].device == a.tensors[0].device, f"k[{i}] must be on the state's device")
+            a.k[i] = ks[i].data_ptr()
+        else:
+            a.k[i] = None
+    a.ks = tuple(ks)                                  # keeps the stage tensors alive with the argument block
+
+
+def ode_stage(a: _lib.OdeArgs, stage: int, ks=()) -> None:
+    """ln3_ode_stage: y_stage and t_rows of DP stage `stage` (1..6, reading f0 and ks[:stage-1]) or of the
+    initial-step probe (stage 0)."""
+    _req(0 <= stage <= 6 and len(ks) >= max(stage - 1, 0), "stage i needs the i-1 previous stage derivatives")
+    _ode_k(a, ks)
+    _lib.check(_lib.lib().ln3_ode_stage(C.byref(a), stage, _lib.current_stream()), "ln3_ode_stage")
+
+
+def ode_initial_step(a: _lib.OdeArgs, phase: int, k0: torch.Tensor | None = None) -> None:
+    """ln3_ode_initial_step: phase 0 -> h0 per group; phase 1 (k0 = forward at the stage-0 probe) -> first dt."""
+    _req(phase in (0, 1) and (phase == 0 or k0 is not None), "phase 1 needs k0")
+    _ode_k(a, () if k0 is None else (k0,))
+    _lib.check(_lib.lib().ln3_ode_initial_step(C.byref(a), phase, _lib.current_stream()), "ln3_ode_initial_step")
+
+
+def ode_step(a: _lib.OdeArgs, ks) -> None:
+    """ln3_ode_step: error ratio, accept / reject, next dt, commit and dense output, from the six stage derivatives."""
+    _req(len(ks) == 6, "ode_step needs the six stage derivatives")
+    _ode_k(a, ks)
+    _lib.check(_lib.lib().ln3_ode_step(C.byref(a), _lib.current_stream()), "ln3_ode_step")
+
+
 def generate_rays(cams: torch.Tensor, res: int):
     """cams fp32 (V,25) -> ray_o, ray_d fp32 (V, res*res, 3) (RaySampler.forward)."""
     _cuda(cams, "cams", torch.float32)

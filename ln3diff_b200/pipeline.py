@@ -207,6 +207,111 @@ def sample_flow(model, c: dict, uc: dict, num_samples: int, seed: int = 42, num_
     return samples.chunk(2, dim=0)[0]
 
 
+def flow_batch_row_groups(P: int, num_samples: int) -> torch.Tensor:
+    """The condition of every row of the batched CFG state cat([zs, zs]) of P conditions x num_samples samples
+    (condition-major): rows [gN, (g+1)N) and [PN + gN, PN + (g+1)N) are condition g.  int32 (2PN,)."""
+    g = torch.arange(P, dtype=torch.int32).repeat_interleave(num_samples)
+    return torch.cat([g, g])
+
+
+def flow_batch_noise(P: int, num_samples: int, shape: tuple, seed: int = 42) -> torch.Tensor:
+    """The initial noise of P conditions, (P*N, *shape) condition-major: each condition gets the draw `sample_flow`
+    makes, `torch.manual_seed(seed); randn(N, *shape)` on the CPU (so all conditions get the same noise, as P
+    sequential calls would).  Seeds the global generators as sample_flow does."""
+    torch.manual_seed(seed)
+    zs = torch.randn(num_samples, *shape)
+    return zs.repeat(P, *([1] * len(shape)))
+
+
+def flow_batch_context(c: dict, uc: dict, dev=None, dtype=torch.float32) -> dict:
+    """The CFG context of `sample_flow` for stacked conditions: cat((c, uc)) per tensor key (conditional rows first),
+    rounded to `dtype` and carried in fp32; other keys must agree between c and uc and are passed through."""
+    ctx = {}
+    for k in c:
+        if k in ("vector", "crossattn", "concat"):
+            ctx[k] = torch.cat((c[k], uc[k]), 0).to(dev).to(dtype).float().contiguous()
+        else:
+            assert c[k] == uc[k]
+            ctx[k] = c[k]
+    return ctx
+
+
+@torch.no_grad()
+def sample_flow_batched(model, c: dict, uc: dict, num_samples: int, seed: int = 42, num_steps: int = 250,
+                        cfg_scale: float = 4.0, dtype=torch.float32):
+    """`sample_flow` with its default dopri5 solver for P conditions in one denoiser batch.  c / uc hold P conditions
+    stacked condition-major, each repeated `num_samples` times as `condition_prompt` returns it ((P*N, ...) per key).
+    The batch is cat([zs, zs]) of 2PN rows with context cat((c, uc)); every condition runs its own adaptive dopri5
+    trajectory (transport/dopri5.py:odeint_dopri5_grouped), so its latents do not depend on the other conditions in
+    the batch.  The noise is `flow_batch_noise` (sample_flow's draw for every condition).  num_steps is the output
+    grid of sample_ode; dopri5 only uses its last point, t = 1.
+    Returns (latents (P, N, 12, 32, 32) fp32, stats) with per-condition lists nfe / accepted / rejected and the
+    batch's forward count batch_nfe."""
+    from .transport.dopri5 import odeint_dopri5_grouped
+    dev = next(model.parameters()).device
+    if dev.type != "cuda":
+        raise RuntimeError("sample_flow_batched runs on CUDA only (no CPU fallback)")
+    N = num_samples
+    rows = next(v for k, v in c.items() if k in ("vector", "crossattn", "concat")).shape[0]
+    assert rows % N == 0, "c must hold num_samples rows per condition"
+    P = rows // N
+    C = 3 * model.in_channels if model.roll_out else model.in_channels
+    shape = (C, model.input_size, model.input_size)
+    zs = flow_batch_noise(P, N, shape, seed).to(dev).to(dtype).float()
+    ctx = flow_batch_context(c, uc, dev, dtype)
+    grid = torch.linspace(0, 1, num_steps)            # sample_ode's grid: dopri5 integrates to its last point
+    fn = lambda t, x: model.forward_with_cfg(x, t, ctx, cfg_scale)
+    y, stats = odeint_dopri5_grouped(fn, torch.cat([zs, zs], 0), flow_batch_row_groups(P, N), P,
+                                     t0=float(grid[0]), t1=float(grid[-1]), rtol=1e-3, atol=1e-6)
+    return y[:P * N].reshape(P, N, *shape), stats
+
+
+@torch.no_grad()
+def _conds_to_3d(conditioner, model, decoder, cond_key, prompts, cameras, num_samples, seed, num_steps, cfg_scale,
+                 resolution, dtype):
+    """`_cond_to_3d` for a list of conditions: the conditioner once per condition, in order, one batched sample,
+    then decode and render of every latent.  The render noise is one device draw for the batch."""
+    dev = next(model.parameters()).device
+    cs, ucs = zip(*(condition_prompt(conditioner, cond_key, p, num_samples, device=dev) for p in prompts))
+    c = {k: torch.cat([ci[k] for ci in cs]) if isinstance(cs[0][k], torch.Tensor) else cs[0][k] for k in cs[0]}
+    uc = {k: torch.cat([ui[k] for ui in ucs]) if isinstance(ucs[0][k], torch.Tensor) else ucs[0][k] for k in ucs[0]}
+    latents, stats = sample_flow_batched(model, c, uc, num_samples, seed=seed, num_steps=num_steps,
+                                         cfg_scale=cfg_scale, dtype=dtype)
+    P, N = latents.shape[:2]
+    out = decode_and_render(decoder, latents.reshape(P * N, *latents.shape[2:]), cameras[:24].to(dev), resolution)
+    return latents, {k: v.reshape(P, N, *v.shape[1:]) for k, v in out.items()}, stats
+
+
+@torch.no_grad()
+def images_to_3d(conditioner, model, decoder, images: torch.Tensor, cameras: torch.Tensor, num_samples: int = 4,
+                 seed: int = 42, num_steps: int = 250, cfg_scale: float = 4.0, resolution: int = 192,
+                 dtype=torch.float32):
+    """`image_to_3d` with dopri5 for P images (P, 3, H, W) in [-1, 1] in one denoiser batch.  Each image's latents
+    are those `image_to_3d` gives for it alone up to the rounding of the batched GEMMs; the renders use one device
+    noise draw for the whole batch, so they are not bit-identical to sequential calls.
+    Returns (latents (P, N, 12, 32, 32), render dict with (P, N, 24, ...) tensors, per-image stats)."""
+    dev = next(model.parameters()).device
+    imgs = [images[i:i + 1].to(dev).to(dtype).clone() for i in range(images.shape[0])]   # own, aligned buffers
+    return _conds_to_3d(conditioner, model, decoder, "img", imgs, cameras, num_samples, seed, num_steps, cfg_scale,
+                        resolution, dtype)
+
+
+@torch.no_grad()
+def mvs_to_3d(conditioner, model, decoder, mv_images: torch.Tensor, mv_cameras: torch.Tensor, cameras: torch.Tensor,
+              num_samples: int = 4, seed: int = 42, num_steps: int = 250, cfg_scale: float = 4.0,
+              resolution: int = 192, dtype=torch.float32):
+    """`mv_to_3d` with dopri5 for P multi-view conditions, mv_images (P, V, 3, H, W) and mv_cameras (P, V, 25), in one
+    denoiser batch.  The conditioner runs once per condition in order, so its `aug_c` camera draws follow the same
+    sequence as P sequential `mv_to_3d` calls.  Every condition gets its own copy of its views and cameras (the
+    conditioner's kernels want 16-byte aligned rows), so with `aug_c=True` the rotations apply to those copies and the
+    caller's `mv_cameras` is left as it is.  Returns as `images_to_3d`."""
+    dev = next(model.parameters()).device
+    own = lambda x, i: x[i:i + 1].to(dev).to(dtype).clone()
+    prompts = [{"img": own(mv_images, i), "c": own(mv_cameras, i)} for i in range(mv_images.shape[0])]
+    return _conds_to_3d(conditioner, model, decoder, "img-c", prompts, cameras, num_samples, seed, num_steps,
+                        cfg_scale, resolution, dtype)
+
+
 @torch.no_grad()
 def _cond_to_3d(conditioner, model, decoder, cond_key, prompt, cameras, num_samples, seed, num_steps, cfg_scale,
                 sampling_method, resolution, dtype):

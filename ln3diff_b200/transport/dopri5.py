@@ -122,3 +122,75 @@ def odeint_dopri5(fn, y0: th.Tensor, t, rtol: float = 1e-3, atol: float = 1e-6, 
     if stats is not None:
         stats.update(nfe=nfe[0], accepted=accepted, rejected=rejected)
     return th.stack(sol, 0)
+
+
+class Dopri5GroupError(RuntimeError):
+    """Raised by `odeint_dopri5_grouped` when a group exceeds max_num_steps or its step underflows.  `groups` lists
+    the failed groups; `y` and `stats` hold the result of the solve, in which every other group is complete."""
+
+    def __init__(self, msg, groups, y, stats):
+        super().__init__(msg)
+        self.groups, self.y, self.stats = groups, y, stats
+
+
+def odeint_dopri5_grouped(fn, y0: th.Tensor, row_group, n_groups: int, t0: float = 0.0, t1: float = 1.0,
+                          rtol: float = 1e-3, atol: float = 1e-6, safety: float = 0.9, ifactor: float = 10.0,
+                          dfactor: float = 0.2, max_num_steps: int = 2 ** 31 - 1):
+    """`odeint_dopri5` for `n_groups` independent problems in one batch, its control logic on the device.
+
+    Row r of y0 (B, ...) fp32 on CUDA belongs to group row_group[r] (int sequence or tensor, every group non-empty).
+    Each group follows exactly the steps `odeint_dopri5(fn_g, y0_g, [t0, ..., t1])` takes for its rows alone (the
+    interior points of a grid never change the step sequence; only the last is an output): its own error norm, step
+    size, accept / reject, counters and end.  fn(t_rows, y) -> dy/dt takes the per-row fp32 time (B,) and returns a
+    new (B, ...) tensor; rows of finished groups keep flowing through it with their state frozen, so the batch shape
+    never changes.  max_num_steps bounds the attempts of a group from t0 to t1.
+
+    The host enqueues attempt n + 2 only after it has read the status of attempt n (copied to pinned memory behind an
+    event), so the GPU never waits on the host and at most one attempt (6 forwards) runs after the last group ends.
+    Returns (y(t1) (B, ...), stats) with per-group lists nfe / accepted / rejected and batch_nfe, the forwards the
+    batch ran.  Raises Dopri5GroupError naming the groups that failed."""
+    from .. import ops
+    if not y0.is_cuda:
+        raise RuntimeError("odeint_dopri5_grouped runs on CUDA only (no CPU fallback)")
+    assert t1 > t0, "t1 must be greater than t0"
+    dev, B = y0.device, y0.shape[0]
+    y = y0.float().contiguous().clone()
+    t_rows = th.full((B,), float(t0), device=dev, dtype=th.float32)
+    f0 = fn(t_rows, y).float().contiguous().clone()
+    y_stage, out = th.empty_like(y), th.full_like(y, float("nan"))
+    state = ops.ode_state(n_groups, t0, dev)
+    rg = th.as_tensor(row_group, dtype=th.int32)
+    a = ops.ode_args(y, f0, y_stage, t_rows, out, rg, state, t_end=float(t1), rtol=rtol, atol=atol, safety=safety,
+                     ifactor=ifactor, dfactor=dfactor, max_num_steps=max_num_steps)
+    ops.ode_initial_step(a, 0)
+    ops.ode_stage(a, 0)
+    ops.ode_initial_step(a, 1, fn(t_rows, y_stage).float().contiguous())
+    batch_nfe = 2
+    pinned = th.empty((2,) + tuple(state.shape), dtype=th.uint8, pin_memory=True)
+    events = [th.cuda.Event(), th.cuda.Event()]
+    n = 0
+    while True:
+        ks = []
+        for i in range(1, 7):
+            ops.ode_stage(a, i, ks)
+            ks.append(fn(t_rows, y_stage).float().contiguous())
+        ops.ode_step(a, ks)
+        batch_nfe += 6
+        pinned[n % 2].copy_(state, non_blocking=True)
+        events[n % 2].record()
+        if n >= 1:                        # attempt n is in flight while the host reads attempt n - 1
+            events[(n - 1) % 2].synchronize()
+            if not bool((ops.ode_state_fields(pinned[(n - 1) % 2])["status"] == 0).any()):
+                break
+        n += 1
+    events[n % 2].synchronize()
+    f = ops.ode_state_fields(pinned[n % 2])
+    stats = dict(nfe=f["nfe"].tolist(), accepted=f["accepted"].tolist(), rejected=f["rejected"].tolist(),
+                 batch_nfe=batch_nfe)
+    failed = [g for g, s in enumerate(f["status"].tolist()) if s < 0]
+    if failed:
+        why = {-1: "max_num_steps exceeded", -2: "underflow in dt"}
+        msg = "; ".join(f"group {g}: {why[int(f['status'][g])]} (t={float(f['t'][g])}, dt={float(f['dt'][g])})"
+                        for g in failed)
+        raise Dopri5GroupError(f"odeint_dopri5_grouped: {msg}", failed, out, stats)
+    return out, stats
