@@ -588,6 +588,82 @@ typedef struct ln3_vae_posterior_args {
 
 int ln3_vae_posterior(const ln3_vae_posterior_args* args, void* stream);
 
+/* ------------------------------------------------------------------ FP8 (e4m3) denoiser GEMMs
+ * An opt-in operating point for the qkv / fc1 / fc2 GEMMs of the DiT blocks.  Its results are NOT held to the
+ * reference's parity tolerance: fp8 operands move the outputs by far more than bf16 rounding does.
+ *
+ * Number format.  Codes are e4m3 with the encoding and the +-448 saturation of torch.float8_e4m3fn.
+ *   Activations: 1 x 128 block scales.  A is e4m3 [M, K] with fp32 a_scale[M, K/128]; block (m, kb) covers
+ *     columns [128 kb, 128 kb + 128) of row m and is quantised as
+ *       s = fp32(absmax / 448)            (IEEE division; an all-zero block has s = 0 and zero codes)
+ *       q = e4m3_rn_satfinite(fp32(x / s))
+ *     so x ~ q * s.  ln3_quantize_fp8_rows, ln3_norm_modulate_fp8 and the LN3_OUT_FP8 epilogue all write this.
+ *   Weights: per output channel.  W is e4m3 [N, K] with fp32 w_scale[N] (quantised once, off the hot path, with
+ *     torch's float8_e4m3fn cast of W / w_scale, w_scale = absmax of the row / 448).
+ *
+ * ln3_gemm_fp8: out = epilogue(w_scale[n] * sum_kb a_scale[m, kb] * P(m, n, kb)),  P = sum_{k in kb} q_a q_w.
+ *   Each 128-deep partial P comes out of the tensor core's fp8 MMA (whose internal accumulation is narrower
+ *   than fp32) in an accumulator of its own and is added, scaled by a_scale, into a separate fp32 accumulator:
+ *   acc = fmaf(a_scale[m, kb], P, acc).  Then y = fmaf(acc, w_scale[n], bias[n]) and one of
+ *     LN3_OUT_BF16 with LN3_ACT_NONE   bf16 [M, ldo], optionally with the per-head RMSNorm of ln3_gemm_args
+ *                                      (head_norm_*, same semantics) before the store
+ *     LN3_OUT_FP8 with LN3_ACT_NONE or LN3_ACT_GELU_ERF (the polynomial of the bf16 GEMM's fc1 epilogue)
+ *                                      e4m3 [M, ldo] with block scales out_scale[M, N/128] (pitch out_scale_ld),
+ *                                      the operand format above, so fc1 writes fc2's A directly.
+ *   Deterministic: no split-K, no atomics; each output sees the same instructions in the same order whatever
+ *   the grid.  LN3_EINVAL unless M > 0, K % 128 == 0, N % 128 == 0, A, W, out 16-byte aligned, lda, ldw and the
+ *   output row pitch in bytes multiples of 16, a_scale and w_scale given, a_scale_ld >= K/128, bias 16-byte
+ *   aligned, and with LN3_OUT_FP8 out_scale given with out_scale_ld >= N/128.  LN3_EUNSUPPORTED for any other
+ *   output kind / activation pairing and for head_norm outside LN3_OUT_BF16.  There is no bf16 fallback.
+ *
+ * ln3_norm_modulate_fp8: ln3_norm_modulate (`base`: the same residual update, norm and modulation, the same
+ *   residual-stream arithmetic bit for bit) writing the e4m3 + block-scale format instead of bf16.  base.out must
+ *   be NULL (base.ldo is ignored).  LN3_EINVAL for the checks of ln3_norm_modulate plus out / out_scale NULL or
+ *   misaligned (out 16 bytes, ldo % 16), out_scale_ld < D/128; LN3_EUNSUPPORTED unless D % 256 == 0, D <= 1536,
+ *   base.ldx % 8 == 0, x 32-byte aligned and (with resid) resid_ld % 8 == 0.
+ *
+ * ln3_quantize_fp8_rows: x (fp32, or bf16 when x_bf16 != 0) [rows, ldx] -> out e4m3 [rows, ldo] + out_scale
+ *   [rows, out_scale_ld].  rows <= 0 returns without a launch; otherwise LN3_EINVAL for a NULL pointer, D not a
+ *   positive multiple of 128, ldx < D, ldo < D or out_scale_ld < D/128, ldx % 4 (fp32) / % 8 (bf16), ldo % 16 or
+ *   x / out not 16-byte aligned.
+ */
+enum { LN3_OUT_FP8 = 3 };
+
+typedef struct ln3_gemm_fp8_args {
+  const void* A;         /* e4m3 [M, lda] */
+  const float* a_scale;  /* [M, a_scale_ld] */
+  const void* W;         /* e4m3 [N, ldw] */
+  const float* w_scale;  /* [N] */
+  const float* bias;     /* [N] or NULL */
+  void* out;             /* bf16 or e4m3 [M, ldo] */
+  float* out_scale;      /* LN3_OUT_FP8: [M, out_scale_ld] */
+  int M, N, K;
+  long long lda, ldw, ldo, a_scale_ld, out_scale_ld;
+  int act;
+  int out_kind;
+  const float* head_norm_w;
+  int head_norm_nsec;
+  int head_norm_sec_cols;
+  float head_norm_eps;
+  /* reserved scratch (ln3_gemm_fp8_workspace_bytes() returns 0); ignored. */
+  void* workspace;
+  size_t workspace_bytes;
+} ln3_gemm_fp8_args;
+
+size_t ln3_gemm_fp8_workspace_bytes(void);
+int ln3_gemm_fp8(const ln3_gemm_fp8_args* args, void* stream);
+
+typedef struct ln3_norm_modulate_fp8_args {
+  ln3_norm_modulate_args base;
+  void* out;         /* e4m3 [rows, ldo] */
+  float* out_scale;  /* [rows, out_scale_ld] */
+  long long ldo, out_scale_ld;
+} ln3_norm_modulate_fp8_args;
+
+int ln3_norm_modulate_fp8(const ln3_norm_modulate_fp8_args* args, void* stream);
+int ln3_quantize_fp8_rows(const void* x, int x_bf16, long long ldx, int rows, int D, void* out, long long ldo,
+                          float* out_scale, long long out_scale_ld, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -15,6 +15,7 @@ LIB_PATH = _PKG / "libln3b200.so"
 LN3_OK = 0
 ACT_NONE, ACT_GELU_ERF, ACT_GELU_TANH, ACT_SILU, ACT_QUICK_GELU = 0, 1, 2, 3, 4
 OUT_BF16, OUT_F32, OUT_RESID_F32 = 0, 1, 2
+OUT_FP8 = 3
 
 _lib = None
 
@@ -59,6 +60,27 @@ class NormModulateArgs(C.Structure):
         ("resid_bcast", C.c_void_p), ("resid_bcast_ld", C.c_longlong), ("resid_bcast_rows", C.c_int),
         ("resid_row_begin", C.c_int), ("resid_row_end", C.c_int),
         ("resid_out_gate", C.c_void_p), ("resid_out_gate_ld", C.c_longlong), ("resid_out_gate_rows", C.c_int),
+    ]
+
+
+class GemmFp8Args(C.Structure):
+    _fields_ = [
+        ("A", C.c_void_p), ("a_scale", C.c_void_p), ("W", C.c_void_p), ("w_scale", C.c_void_p),
+        ("bias", C.c_void_p), ("out", C.c_void_p), ("out_scale", C.c_void_p),
+        ("M", C.c_int), ("N", C.c_int), ("K", C.c_int),
+        ("lda", C.c_longlong), ("ldw", C.c_longlong), ("ldo", C.c_longlong),
+        ("a_scale_ld", C.c_longlong), ("out_scale_ld", C.c_longlong),
+        ("act", C.c_int), ("out_kind", C.c_int),
+        ("head_norm_w", C.c_void_p), ("head_norm_nsec", C.c_int), ("head_norm_sec_cols", C.c_int),
+        ("head_norm_eps", C.c_float),
+        ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t),
+    ]
+
+
+class NormModulateFp8Args(C.Structure):
+    _fields_ = [
+        ("base", NormModulateArgs), ("out", C.c_void_p), ("out_scale", C.c_void_p),
+        ("ldo", C.c_longlong), ("out_scale_ld", C.c_longlong),
     ]
 
 
@@ -202,6 +224,9 @@ def lib() -> C.CDLL:
         L.ln3_add_launch_count.restype = None
         L.ln3_render_workspace_bytes.restype = C.c_size_t
         L.ln3_gemm_workspace_bytes.restype = C.c_size_t
+        L.ln3_gemm_fp8_workspace_bytes.restype = C.c_size_t
+        L.ln3_quantize_fp8_rows.argtypes = [C.c_void_p, C.c_int, C.c_longlong, C.c_int, C.c_int, C.c_void_p,
+                                            C.c_longlong, C.c_void_p, C.c_longlong, C.c_void_p]
         L.ln3_marching_cubes_workspace_bytes.restype = C.c_size_t
         L.ln3_ode_workspace_bytes.restype = C.c_size_t
         L.ln3_ode_workspace_bytes.argtypes = [C.c_int, C.c_longlong]

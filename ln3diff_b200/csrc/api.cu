@@ -94,6 +94,24 @@ int make_tmap_2d_bf16(CUtensorMap* out, const void* ptr, long long rows, long lo
   return LN3_OK;
 }
 
+int make_tmap_2d_u8(CUtensorMap* out, const void* ptr, long long rows, long long cols, long long ld, int box_rows,
+                    int box_cols) {
+  EncodeTiledFn fn = get_encode_fn();
+  if (!fn) return LN3_ECUDA;
+  if (box_cols != 128) return set_error(LN3_EINVAL, "tmap: box_cols must be 128 (128B swizzle)");
+  cuuint64_t dims[2] = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(rows)};
+  cuuint64_t strides[1] = {static_cast<cuuint64_t>(ld)};
+  cuuint32_t box[2] = {static_cast<cuuint32_t>(box_cols), static_cast<cuuint32_t>(box_rows)};
+  cuuint32_t estr[2] = {1, 1};
+  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<void*>(ptr), dims, strides, box, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS)
+    return set_error(LN3_ECUDA, "cuTensorMapEncodeTiled(2d u8 rows=%lld cols=%lld ld=%lld) -> %d", rows, cols, ld,
+                     static_cast<int>(r));
+  return LN3_OK;
+}
+
 int make_tmap_3d_bf16(CUtensorMap* out, const void* ptr, long long d0, long long d1, long long d2,
                       long long s1, long long s2, int box0, int box1) {
   EncodeTiledFn fn = get_encode_fn();
@@ -292,6 +310,22 @@ int ln3_ode_step(const ln3_ode_args* args, void* stream) {
   int rc = ode_validate(args, ODE_NEED_STAGE | ODE_NEED_K | ODE_NEED_OUT | ODE_NEED_WS, "ode_step");
   if (rc != LN3_OK) return rc;
   return ode_step(args, static_cast<cudaStream_t>(stream));
+}
+
+
+size_t ln3_gemm_fp8_workspace_bytes(void) { return gemm_fp8_workspace_bytes(); }
+int ln3_gemm_fp8(const ln3_gemm_fp8_args* args, void* stream) {
+  if (!args) return set_error(LN3_EINVAL, "gemm_fp8: null args");
+  return gemm_fp8(args, static_cast<cudaStream_t>(stream));
+}
+int ln3_norm_modulate_fp8(const ln3_norm_modulate_fp8_args* args, void* stream) {
+  if (!args) return set_error(LN3_EINVAL, "norm_modulate_fp8: null args");
+  return norm_modulate_fp8(args, static_cast<cudaStream_t>(stream));
+}
+int ln3_quantize_fp8_rows(const void* x, int x_bf16, long long ldx, int rows, int D, void* out, long long ldo,
+                          float* out_scale, long long out_scale_ld, void* stream) {
+  return quantize_fp8_rows(x, x_bf16, ldx, rows, D, out, ldo, out_scale, out_scale_ld,
+                           static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

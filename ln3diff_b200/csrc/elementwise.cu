@@ -1,5 +1,6 @@
 // HBM-bound glue kernels of the DiT / sampler path (fp32 SIMT, vectorised, coalesced):
-//   norm_modulate      LayerNorm/RMSNorm + adaLN modulate -> bf16 GEMM operand
+//   norm_modulate      LayerNorm/RMSNorm + adaLN modulate -> bf16 GEMM operand (or e4m3 + block scales: _fp8)
+//   quantize_fp8_rows  fp32 / bf16 rows -> e4m3 codes + 1 x 128 block scales
 //   timestep_embedding sinusoidal features of the timestep
 //   patch_embed        roll-out rearrange + 2x2 patch conv + pos_embed -> fp32 token stream
 //   final_layer        LN + modulate + Linear(D -> 4*Cout) + unpatchify -> fp32 latent layout
@@ -160,9 +161,45 @@ __device__ __forceinline__ bool nm_needs_own_row(const ln3_norm_modulate_args& a
 // LN3_RESID_L2=1: residual-stream accesses carry the L2 evict_last priority (set once per process)
 __constant__ int c_nm_l2_hint;
 
-template <int NV8>
+// Outputs of the row body: `enabled()` is false for a residual-only pass; `store(row, lane, c, y)` writes the 8
+// normalised values of columns [c, c + 8), called by all 32 lanes for the same chunk index.
+struct NmOutBf16 {
+  void* out;
+  long long ldo;
+  __device__ __forceinline__ bool enabled() const { return out != nullptr; }
+  __device__ __forceinline__ void store(int row, int, int c, const float (&y)[8]) const {
+    uint4 pk;
+    pk.x = pack_bf16x2(y[0], y[1]);
+    pk.y = pack_bf16x2(y[2], y[3]);
+    pk.z = pack_bf16x2(y[4], y[5]);
+    pk.w = pack_bf16x2(y[6], y[7]);
+    *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(out) + static_cast<long long>(row) * ldo + c) = pk;
+  }
+};
+// e4m3 codes + 1 x 128 block scales (include/ln3b200.h): a 128-column block is chunk i of 16 consecutive lanes
+struct NmOutFp8 {
+  void* out;
+  float* out_scale;
+  long long ldo, out_scale_ld;
+  __device__ __forceinline__ bool enabled() const { return true; }
+  __device__ __forceinline__ void store(int row, int lane, int c, const float (&y)[8]) const {
+    float amax = 0.f;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) amax = fmaxf(amax, fabsf(y[j]));
+#pragma unroll
+    for (int o = 1; o < 16; o <<= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+    const float s = fp8_block_scale(amax);
+    uint2 pk;
+    pk.x = fp8_code2(y[0], y[1], s) | (static_cast<uint32_t>(fp8_code2(y[2], y[3], s)) << 16);
+    pk.y = fp8_code2(y[4], y[5], s) | (static_cast<uint32_t>(fp8_code2(y[6], y[7], s)) << 16);
+    *reinterpret_cast<uint2*>(reinterpret_cast<uint8_t*>(out) + static_cast<long long>(row) * ldo + c) = pk;
+    if ((lane & 15) == 0) out_scale[static_cast<long long>(row) * out_scale_ld + c / 128] = s;
+  }
+};
+
+template <int NV8, class Out>
 __device__ __forceinline__ void nm_row_body(const ln3_norm_modulate_args& a, int row, int lane, float (&v)[NV8][8],
-                                            const uint4 (&rown)[NV8]) {
+                                            const uint4 (&rown)[NV8], const Out& out) {
   float* x = const_cast<float*>(a.x) + static_cast<long long>(row) * a.ldx;
   auto ld8 = [&](const float* p8, float* d8) {
     const float4 p0 = __ldg(reinterpret_cast<const float4*>(p8));
@@ -212,7 +249,7 @@ __device__ __forceinline__ void nm_row_body(const ln3_norm_modulate_args& a, int
       if (c_nm_l2_hint) stg256_f32_el(x + c, v[i]);
       else stg256_f32(x + c, v[i]);
     }
-    if (a.out == nullptr) return;
+    if (!out.enabled()) return;
   }
   float mean = 0.f, rstd = 1.f;
   if (a.norm == LN3_NORM_LAYER) {
@@ -245,7 +282,6 @@ __device__ __forceinline__ void nm_row_body(const ln3_norm_modulate_args& a, int
     sh = a.shift + g * a.mod_ld;
     sc = a.scale + g * a.mod_ld;
   }
-  __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(a.out) + static_cast<long long>(row) * a.ldo;
 #pragma unroll
   for (int i = 0; i < NV8; ++i) {
     const int c = (i * 32 + lane) * 8;
@@ -276,12 +312,7 @@ __device__ __forceinline__ void nm_row_body(const ln3_norm_modulate_args& a, int
 #pragma unroll
       for (int j = 0; j < 8; ++j) y[j] = apply_act(y[j], a.act);
     }
-    uint4 pk;
-    pk.x = pack_bf16x2(y[0], y[1]);
-    pk.y = pack_bf16x2(y[2], y[3]);
-    pk.z = pack_bf16x2(y[4], y[5]);
-    pk.w = pack_bf16x2(y[6], y[7]);
-    *reinterpret_cast<uint4*>(o + c) = pk;
+    out.store(row, lane, c, y);
   }
 }
 
@@ -309,9 +340,9 @@ __device__ __forceinline__ void nm_load_row(const ln3_norm_modulate_args& a, int
   }
 }
 
-template <int NV8>
+template <int NV8, class Out>
 __global__ void __launch_bounds__(256, 3)
-norm_modulate_wide_kernel(const ln3_norm_modulate_args a) {
+norm_modulate_wide_kernel(const ln3_norm_modulate_args a, const Out out) {
   pdl_launch_dependents();
   pdl_wait();
   const int lane = threadIdx.x & 31;
@@ -325,7 +356,7 @@ norm_modulate_wide_kernel(const ln3_norm_modulate_args a) {
     float v[NV8][8];
     uint4 rown[NV8];
     nm_load_row<NV8>(a, row, lane, v, rown);
-    nm_row_body<NV8>(a, row, lane, v, rown);
+    nm_row_body<NV8>(a, row, lane, v, rown, out);
   }
 }
 
@@ -333,8 +364,8 @@ norm_modulate_wide_kernel(const ln3_norm_modulate_args a) {
 // column-offset view such as mod[:, 1:1+D] would otherwise pass the shape checks and issue misaligned loads.
 static bool misaligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) != 0; }
 
-int norm_modulate(const ln3_norm_modulate_args* a, cudaStream_t stream) {
-  if (a->rows <= 0) return LN3_OK;
+// Argument checks of the norm_modulate entry points; `out` / `ldo` are the output this call writes.
+static int nm_check(const ln3_norm_modulate_args* a, const void* out, long long ldo) {
   if (a->D % 128 != 0 || a->D > 2048 || a->D <= 0)
     return set_error(LN3_EINVAL, "norm_modulate: D=%d must be a multiple of 128, <= 2048", a->D);
   if ((a->shift == nullptr) != (a->scale == nullptr))
@@ -343,11 +374,11 @@ int norm_modulate(const ln3_norm_modulate_args* a, cudaStream_t stream) {
     return set_error(LN3_EINVAL, "norm_modulate: shift_tab and scale_tab must be given together");
   if (a->shift != nullptr && a->mod_rows <= 0)
     return set_error(LN3_EINVAL, "norm_modulate: mod_rows must be > 0");
-  if (a->ldx % 4 || a->ldo % 4 || (a->shift && a->mod_ld % 4))
+  if (a->ldx % 4 || ldo % 4 || (a->shift && a->mod_ld % 4))
     return set_error(LN3_EINVAL, "norm_modulate: leading dimensions must be multiples of 4");
-  if (a->out == nullptr && a->resid == nullptr) return set_error(LN3_EINVAL, "norm_modulate: out is NULL");
+  if (out == nullptr && a->resid == nullptr) return set_error(LN3_EINVAL, "norm_modulate: out is NULL");
   // out and resid need only 8 bytes in the float4 kernel and 16 in the 256-bit one: one rule, the stricter
-  if (misaligned16(a->x) || misaligned16(a->out) || misaligned16(a->shift) || misaligned16(a->scale) ||
+  if (misaligned16(a->x) || misaligned16(out) || misaligned16(a->shift) || misaligned16(a->scale) ||
       misaligned16(a->shift_tab) || misaligned16(a->scale_tab) || misaligned16(a->weight) || misaligned16(a->resid) ||
       misaligned16(a->resid_gate) || misaligned16(a->resid_bcast) || misaligned16(a->resid_out_gate))
     return set_error(LN3_EINVAL, "norm_modulate: x, out, shift, scale, tables, weight, resid, resid_bcast and gates must be 16-byte aligned");
@@ -365,40 +396,57 @@ int norm_modulate(const ln3_norm_modulate_args* a, cudaStream_t stream) {
   } else if (a->resid_bcast != nullptr) {
     return set_error(LN3_EINVAL, "norm_modulate: resid_bcast needs resid");
   }
-  const int warps = 8;
-  const int blocks_needed = (a->rows + warps - 1) / warps;
+  return LN3_OK;
+}
+
+// x, ldx and resid as the 256-bit kernels need them (D itself is checked by the caller)
+static bool nm_wide_input(const ln3_norm_modulate_args* a) {
+  return a->ldx % 8 == 0 && (reinterpret_cast<uintptr_t>(a->x) & 31) == 0 &&
+         (a->resid == nullptr || (a->resid_ld % 8 == 0 && (reinterpret_cast<uintptr_t>(a->resid) & 15) == 0));
+}
+
+static int nm_l2_hint_once() {  // LN3_RESID_L2=1: evict_last hints on the residual stream (uploaded once per device)
+  static DeviceOnce l2_once;
+  return l2_once.run([] {
+    const int v = (getenv("LN3_RESID_L2") && atoi(getenv("LN3_RESID_L2")) != 0) ? 1 : 0;
+    cudaError_t e = cudaMemcpyToSymbol(c_nm_l2_hint, &v, sizeof(v));
+    return e == cudaSuccess ? LN3_OK : set_error(LN3_ECUDA, "norm_modulate: constant upload: %s", cudaGetErrorString(e));
+  });
+}
+
+static constexpr int kNmWarps = 8;
+
+template <class Out>
+static int nm_launch_wide(const ln3_norm_modulate_args* a, const Out& out, cudaStream_t stream) {
+  const int blocks_needed = (a->rows + kNmWarps - 1) / kNmWarps;
+  const int wave3 = device_sm_count() * 3;  // 3 resident blocks per SM at <= 80 registers
+  const dim3 grid(blocks_needed < wave3 ? blocks_needed : wave3), block(kNmWarps * 32);
+  cudaError_t le = cudaSuccess;
+  switch (a->D / 256) {
+    case 1: le = launch_pdl(norm_modulate_wide_kernel<1, Out>, grid, block, 0, stream, *a, out); break;
+    case 2: le = launch_pdl(norm_modulate_wide_kernel<2, Out>, grid, block, 0, stream, *a, out); break;
+    case 3: le = launch_pdl(norm_modulate_wide_kernel<3, Out>, grid, block, 0, stream, *a, out); break;
+    case 4: le = launch_pdl(norm_modulate_wide_kernel<4, Out>, grid, block, 0, stream, *a, out); break;
+    case 5: le = launch_pdl(norm_modulate_wide_kernel<5, Out>, grid, block, 0, stream, *a, out); break;
+    default: le = launch_pdl(norm_modulate_wide_kernel<6, Out>, grid, block, 0, stream, *a, out); break;
+  }
+  cudaError_t e = le != cudaSuccess ? le : cudaGetLastError();
+  if (e != cudaSuccess) return set_error(LN3_ECUDA, "norm_modulate launch: %s", cudaGetErrorString(e));
+  count_launch();
+  return LN3_OK;
+}
+
+int norm_modulate(const ln3_norm_modulate_args* a, cudaStream_t stream) {
+  if (a->rows <= 0) return LN3_OK;
+  if (int rc = nm_check(a, a->out, a->ldo)) return rc;
+  const int blocks_needed = (a->rows + kNmWarps - 1) / kNmWarps;
   const int wave = device_sm_count() * 4;  // 4 x 256-thread blocks resident per SM (<= 64 regs/thread)
-  dim3 grid(blocks_needed < wave ? blocks_needed : wave), block(warps * 32);
+  dim3 grid(blocks_needed < wave ? blocks_needed : wave), block(kNmWarps * 32);
   static const bool wide_enabled = !(getenv("LN3_NORM_WIDE") && atoi(getenv("LN3_NORM_WIDE")) == 0);
-  const bool wide = wide_enabled && a->D % 256 == 0 && a->D <= 1536 && a->ldx % 8 == 0 && a->ldo % 8 == 0 &&
-                    (reinterpret_cast<uintptr_t>(a->x) & 31) == 0 && (a->out == nullptr || (reinterpret_cast<uintptr_t>(a->out) & 15) == 0) &&
-                    (a->resid == nullptr || (a->resid_ld % 8 == 0 && (reinterpret_cast<uintptr_t>(a->resid) & 15) == 0));
-  {  // LN3_RESID_L2=1: evict_last hints on the residual stream (uploaded once per device)
-    static DeviceOnce l2_once;
-    if (int rc = l2_once.run([] {
-          const int v = (getenv("LN3_RESID_L2") && atoi(getenv("LN3_RESID_L2")) != 0) ? 1 : 0;
-          cudaError_t e = cudaMemcpyToSymbol(c_nm_l2_hint, &v, sizeof(v));
-          return e == cudaSuccess ? LN3_OK : set_error(LN3_ECUDA, "norm_modulate: constant upload: %s", cudaGetErrorString(e));
-        }))
-      return rc;
-  }
-  if (wide) {
-    cudaError_t le = cudaSuccess;
-    const int wave3 = device_sm_count() * 3;  // 3 resident blocks per SM at <= 80 registers
-    grid = dim3(blocks_needed < wave3 ? blocks_needed : wave3);
-    switch (a->D / 256) {
-      case 1: le = launch_pdl(norm_modulate_wide_kernel<1>, grid, block, 0, stream, *a); break;
-      case 2: le = launch_pdl(norm_modulate_wide_kernel<2>, grid, block, 0, stream, *a); break;
-      case 3: le = launch_pdl(norm_modulate_wide_kernel<3>, grid, block, 0, stream, *a); break;
-      case 4: le = launch_pdl(norm_modulate_wide_kernel<4>, grid, block, 0, stream, *a); break;
-      case 5: le = launch_pdl(norm_modulate_wide_kernel<5>, grid, block, 0, stream, *a); break;
-      default: le = launch_pdl(norm_modulate_wide_kernel<6>, grid, block, 0, stream, *a); break;
-    }
-    cudaError_t e = le != cudaSuccess ? le : cudaGetLastError();
-    if (e != cudaSuccess) return set_error(LN3_ECUDA, "norm_modulate launch: %s", cudaGetErrorString(e));
-    count_launch();
-    return LN3_OK;
-  }
+  const bool wide = wide_enabled && a->D % 256 == 0 && a->D <= 1536 && a->ldo % 8 == 0 && nm_wide_input(a) &&
+                    (a->out == nullptr || (reinterpret_cast<uintptr_t>(a->out) & 15) == 0);
+  if (int rc = nm_l2_hint_once()) return rc;
+  if (wide) return nm_launch_wide(a, NmOutBf16{a->out, a->ldo}, stream);
   switch (a->D / 128) {
 #define LN3_NM_CASE(n) \
   case n: norm_modulate_kernel<n><<<grid, block, 0, stream>>>(*a); break;
@@ -410,6 +458,77 @@ int norm_modulate(const ln3_norm_modulate_args* a, cudaStream_t stream) {
   }
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error(LN3_ECUDA, "norm_modulate launch: %s", cudaGetErrorString(e));
+  count_launch();
+  return LN3_OK;
+}
+
+// The fp8 output exists for the 256-bit kernels only (every DiT-L/2 and DiT-B/2 width); other shapes are refused.
+int norm_modulate_fp8(const ln3_norm_modulate_fp8_args* f, cudaStream_t stream) {
+  const ln3_norm_modulate_args* a = &f->base;
+  if (a->out != nullptr) return set_error(LN3_EINVAL, "norm_modulate_fp8: base.out must be NULL (the output is out)");
+  if (f->out == nullptr || f->out_scale == nullptr)
+    return set_error(LN3_EINVAL, "norm_modulate_fp8: out and out_scale must be given");
+  if (a->rows <= 0) return LN3_OK;
+  if (int rc = nm_check(a, f->out, f->ldo)) return rc;
+  if (f->ldo < a->D || f->ldo % 16 != 0 || f->out_scale_ld < a->D / 128)
+    return set_error(LN3_EINVAL, "norm_modulate_fp8: ldo must be >= D and a multiple of 16, out_scale_ld >= D/128");
+  if (a->D % 256 != 0 || a->D > 1536 || !nm_wide_input(a))
+    return set_error(LN3_EUNSUPPORTED,
+                     "norm_modulate_fp8: needs D %% 256 == 0, D <= 1536, ldx %% 8 == 0, x 32-byte aligned and "
+                     "resid_ld %% 8 == 0 (D=%d)", a->D);
+  if (int rc = nm_l2_hint_once()) return rc;
+  return nm_launch_wide(a, NmOutFp8{f->out, f->out_scale, f->ldo, f->out_scale_ld}, stream);
+}
+
+// ------------------------------------------------------------------ fp8 block quantisation
+// One warp per 128-column block of a row: 4 consecutive values per lane, the absmax over the warp.
+template <typename T>
+__global__ void __launch_bounds__(256)
+quantize_fp8_kernel(const T* __restrict__ x, long long ldx, int rows, int nblk, uint8_t* __restrict__ out,
+                    long long ldo, float* __restrict__ out_scale, long long out_scale_ld) {
+  const long long w = static_cast<long long>(blockIdx.x) * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (w >= static_cast<long long>(rows) * nblk) return;
+  const int lane = threadIdx.x & 31;
+  const int row = static_cast<int>(w / nblk), c = static_cast<int>(w % nblk) * 128 + lane * 4;
+  float v[4];
+  if constexpr (sizeof(T) == 4) {
+    const float4 t = *reinterpret_cast<const float4*>(x + row * ldx + c);
+    v[0] = t.x, v[1] = t.y, v[2] = t.z, v[3] = t.w;
+  } else {
+    const uint2 t = *reinterpret_cast<const uint2*>(x + row * ldx + c);
+    const __nv_bfloat162 lo = *reinterpret_cast<const __nv_bfloat162*>(&t.x);
+    const __nv_bfloat162 hi = *reinterpret_cast<const __nv_bfloat162*>(&t.y);
+    v[0] = __low2float(lo), v[1] = __high2float(lo), v[2] = __low2float(hi), v[3] = __high2float(hi);
+  }
+  float amax = fmaxf(fmaxf(fabsf(v[0]), fabsf(v[1])), fmaxf(fabsf(v[2]), fabsf(v[3])));
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+  const float s = fp8_block_scale(amax);
+  *reinterpret_cast<uint32_t*>(out + row * ldo + c) =
+      fp8_code2(v[0], v[1], s) | (static_cast<uint32_t>(fp8_code2(v[2], v[3], s)) << 16);
+  if (lane == 0) out_scale[row * out_scale_ld + c / 128] = s;
+}
+
+int quantize_fp8_rows(const void* x, int x_bf16, long long ldx, int rows, int D, void* out, long long ldo,
+                      float* out_scale, long long out_scale_ld, cudaStream_t stream) {
+  if (rows <= 0) return LN3_OK;
+  if (x == nullptr || out == nullptr || out_scale == nullptr)
+    return set_error(LN3_EINVAL, "quantize_fp8_rows: null pointer");
+  if (D <= 0 || D % 128 != 0) return set_error(LN3_EINVAL, "quantize_fp8_rows: D=%d must be a positive multiple of 128", D);
+  if (ldx < D || ldo < D || out_scale_ld < D / 128)
+    return set_error(LN3_EINVAL, "quantize_fp8_rows: ldx and ldo must be >= D, out_scale_ld >= D/128");
+  if (ldx % (x_bf16 ? 8 : 4) != 0 || ldo % 16 != 0 || misaligned16(x) || misaligned16(out))
+    return set_error(LN3_EINVAL, "quantize_fp8_rows: x and out must be 16-byte aligned with 16-byte row pitches");
+  const long long warps = static_cast<long long>(rows) * (D / 128);
+  const dim3 grid(static_cast<unsigned>((warps + 7) / 8)), block(256);
+  if (x_bf16)
+    quantize_fp8_kernel<<<grid, block, 0, stream>>>(static_cast<const __nv_bfloat16*>(x), ldx, rows, D / 128,
+                                                   static_cast<uint8_t*>(out), ldo, out_scale, out_scale_ld);
+  else
+    quantize_fp8_kernel<<<grid, block, 0, stream>>>(static_cast<const float*>(x), ldx, rows, D / 128,
+                                                   static_cast<uint8_t*>(out), ldo, out_scale, out_scale_ld);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return set_error(LN3_ECUDA, "quantize_fp8_rows launch: %s", cudaGetErrorString(e));
   count_launch();
   return LN3_OK;
 }

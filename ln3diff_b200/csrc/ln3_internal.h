@@ -65,7 +65,16 @@ int make_tmap_2d_bf16(CUtensorMap* out, const void* ptr, long long rows, long lo
 int make_tmap_3d_bf16(CUtensorMap* out, const void* ptr, long long d0, long long d1, long long d2,
                       long long s1, long long s2, int box0, int box1);
 
+// 2-D byte (e4m3) tensor map: [rows, cols] with row pitch `ld` bytes, box [box_rows, 128], 128-byte swizzle.
+int make_tmap_2d_u8(CUtensorMap* out, const void* ptr, long long rows, long long cols, long long ld, int box_rows,
+                    int box_cols);
+
 int gemm_bf16(const ln3_gemm_args* a, cudaStream_t stream);
+size_t gemm_fp8_workspace_bytes();
+int gemm_fp8(const ln3_gemm_fp8_args* a, cudaStream_t stream);
+int norm_modulate_fp8(const ln3_norm_modulate_fp8_args* a, cudaStream_t stream);
+int quantize_fp8_rows(const void* x, int x_bf16, long long ldx, int rows, int D, void* out, long long ldo,
+                      float* out_scale, long long out_scale_ld, cudaStream_t stream);
 size_t gemm_workspace_bytes();
 int fmha_fwd(const ln3_fmha_args* a, cudaStream_t stream);
 int norm_modulate(const ln3_norm_modulate_args* a, cudaStream_t stream);

@@ -90,11 +90,23 @@ def run_blocks(blocks: list, cx: dict, ws: dict, x2: torch.Tensor, mods, heads: 
     # norm kernel applies x += gate * val while it reads x anyway (one coalesced pass instead of a
     # thread-per-row read-modify-write in the GEMM epilogue).
     val, pend_gate = ws["v"], None
+    # fp8 precision (set_gemm_precision): qkv / fc1 / fc2 read e4m3 operands with block scales, written by the norm
+    # passes that precede qkv and fc1 and by fc1's epilogue; every other launch is the same as in bf16
+    fp8 = "a8" in ws
+    if fp8:
+        a8 = dict(out=ws["a8"], out_scale=ws["a8s"])
+        norm_a = lambda **kw: ops.norm_modulate_fp8(x2, **a8, **kw)
+    else:
+        norm_a = lambda **kw: ops.norm_modulate(x2, out=ws["a"], **kw)
     for l, (W, mod, (k, v), (k2, v2)) in enumerate(zip(blocks, mods, cx["kv"], dkv)):
         sl = lambda j: mod[:, j * D:(j + 1) * D]
-        ops.norm_modulate(x2, **_pre_norm(W, "n1_w"), shift=sl(0), scale=sl(1), mod_rows=T, out=ws["a"],
-                          resid=val if l > 0 else None, resid_gate=pend_gate, resid_gate_rows=T)
-        ops.gemm(ws["a"], W["qkv_w"], W["qkv_b"], out=ws["qkv"], head_norm=W.get("qk_norm"), head_norm_sec_cols=D)
+        norm_a(**_pre_norm(W, "n1_w"), shift=sl(0), scale=sl(1), mod_rows=T,
+               resid=val if l > 0 else None, resid_gate=pend_gate, resid_gate_rows=T)
+        if fp8:
+            ops.gemm_fp8(ws["a8"], ws["a8s"], W["qkv_q"], W["qkv_s"], W["qkv_b"], out=ws["qkv"],
+                         head_norm=W.get("qk_norm"), head_norm_sec_cols=D)
+        else:
+            ops.gemm(ws["a"], W["qkv_w"], W["qkv_b"], out=ws["qkv"], head_norm=W.get("qk_norm"), head_norm_sec_cols=D)
         ops.fmha(qkv3[:, :, :D], qkv3[:, :, D:2 * D], qkv3[:, :, 2 * D:], heads, out=att3, k2=k2, v2=v2)
         ops.gemm(ws["att"], W["proj_w"], W["proj_b"], out=val)
         if split:
@@ -108,12 +120,17 @@ def run_blocks(blocks: list, cx: dict, ws: dict, x2: torch.Tensor, mods, heads: 
             ops.fmha(q3[g0:g1], k[g0:g1], v[g0:g1], heads, out=att3[g0:g1])
             ops.gemm(ws["att"][r0:r1], W["co_w"], W["co_b"], out=val[r0:r1])
         # x += cross_attn (no gate) ; a = modulate(norm(x)).  Identical-token samples take the closed form.
-        ops.norm_modulate(x2, **_pre_norm(W, "n2_w"), shift=sl(3), scale=sl(4), mod_rows=T, out=ws["a"], resid=val,
-                          resid_bcast=oconst[l] if oconst is not None else None, resid_bcast_rows=T,
-                          resid_rows=(r0, r1) if oconst is not None else None,
-                          resid_out_gate=sl(2) if split else None, resid_out_gate_rows=T)
-        ops.gemm(ws["a"], W["fc1_w"], W["fc1_b"], act=ops.ACT_GELU_ERF, out=ws["h"])
-        ops.gemm(ws["h"], W["fc2_w"], W["fc2_b"], out=val)
+        norm_a(**_pre_norm(W, "n2_w"), shift=sl(3), scale=sl(4), mod_rows=T, resid=val,
+               resid_bcast=oconst[l] if oconst is not None else None, resid_bcast_rows=T,
+               resid_rows=(r0, r1) if oconst is not None else None,
+               resid_out_gate=sl(2) if split else None, resid_out_gate_rows=T)
+        if fp8:
+            ops.gemm_fp8(ws["a8"], ws["a8s"], W["fc1_q"], W["fc1_s"], W["fc1_b"], act=ops.ACT_GELU_ERF,
+                         out_kind=ops.OUT_FP8, out=ws["h8"], out_scale=ws["h8s"])
+            ops.gemm_fp8(ws["h8"], ws["h8s"], W["fc2_q"], W["fc2_s"], W["fc2_b"], out=val)
+        else:
+            ops.gemm(ws["a"], W["fc1_w"], W["fc1_b"], act=ops.ACT_GELU_ERF, out=ws["h"])
+            ops.gemm(ws["h"], W["fc2_w"], W["fc2_b"], out=val)
         pend_gate = sl(5)
     ops.norm_modulate(x2, norm=NORM_NONE, resid=val, resid_gate=pend_gate, resid_gate_rows=T, want_out=False)
 
@@ -133,6 +150,24 @@ class DenoiserMixin:
     conditioning of a context), `_mod_workspace` (its modulation buffers) and `_forward_impl`."""
 
     _ln3_fused_in_scale = False  # forward(..., in_scale=) folds the denoiser's c_in into the patch embed
+    _gemm_precision = "bf16"     # "fp8": see set_gemm_precision
+
+    def set_gemm_precision(self, precision: str):
+        """Operand precision of every block's qkv / fc1 / fc2 GEMMs: "bf16" (the default, held to the reference's
+        parity tolerance) or "fp8" (e4m3 operands with 1x128 activation block scales and per-channel weight scales
+        on the fp8 tensor cores, format in include/ln3b200.h -- faster, and OUTSIDE the parity tolerance).  The
+        parameters and state_dict are untouched; the derived state (repacks, workspaces, conditioning cache, CUDA
+        graphs) is dropped and rebuilt for the new precision on the next forward.  Returns self."""
+        if precision not in ("bf16", "fp8"):
+            raise ValueError(f"gemm precision must be 'bf16' or 'fp8', got {precision!r}")
+        if precision != self.gemm_precision:
+            self._gemm_precision = precision
+            self._invalidate()
+        return self
+
+    @property
+    def gemm_precision(self) -> str:
+        return self._gemm_precision
 
     def initialize_weights(self, zeroed=()):
         """reference dit_models_xformers.py:786-819: xavier-uniform Linears with zero bias, the patch embed as a
@@ -198,12 +233,26 @@ class DenoiserMixin:
             fc1_w=bf(b.mlp.mlp[0].weight), fc1_b=f32(b.mlp.mlp[1].bias),
             fc2_w=bf(b.mlp.mlp[2].weight), fc2_b=f32(b.mlp.mlp[3].bias),
             **self._pack_block(b, bf, f32)) for b in self.blocks]
+        if self.gemm_precision == "fp8":
+            self._check_fp8_shapes()
+            for W, b in zip(P["blocks"], self.blocks):
+                for key, lin in (("qkv", b.attn.qkv), ("fc1", b.mlp.mlp[0]), ("fc2", b.mlp.mlp[2])):
+                    W[key + "_q"], W[key + "_s"] = ops.quantize_weight_fp8(lin.weight.to(dev))
         self._invalidate()
         self._prep = P
         return P
 
     def _pack_block(self, b, bf, f32) -> dict:
         return {}
+
+    def _check_fp8_shapes(self):
+        """The fp8 kernels' shape rules (include/ln3b200.h), checked once so that an unsupported model fails in
+        prepare() with the reason rather than in the middle of a forward."""
+        D = self.embed_dim
+        H = int(self.mlp_ratio) * D
+        if D % 256 != 0 or D > 1536 or H % 128 != 0:
+            raise RuntimeError(f"fp8 GEMM precision needs embed_dim % 256 == 0, embed_dim <= 1536 and an MLP width "
+                               f"% 128 == 0 (embed_dim {D}, MLP width {H}); use set_gemm_precision('bf16')")
 
     def _static(self, key, make):
         st = self._ctx_static.get(key)
@@ -221,6 +270,10 @@ class DenoiserMixin:
             ws = self._ws[B] = dict(tfeat=e(B, 256), th=e(B, D), st=e(B, D), x=e(B, T, D, dt=torch.float32),
                                     xb=e(M, D), a=e(M, D), v=e(M, D), qkv=e(M, 3 * D), att=e(M, D), q=e(M, D),
                                     h=e(M, int(self.mlp_ratio) * D), **self._mod_workspace(B, e))
+            if self.gemm_precision == "fp8":
+                H = int(self.mlp_ratio) * D
+                ws.update(a8=e(M, D, dt=ops.FP8), a8s=e(M, D // 128, dt=torch.float32),
+                          h8=e(M, H, dt=ops.FP8), h8s=e(M, H // 128, dt=torch.float32))
         return ws
 
     def _graph(self, B, cx, shared_mod: bool = False) -> ForwardGraph:

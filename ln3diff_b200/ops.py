@@ -12,11 +12,14 @@ import ctypes as C
 import torch
 
 from . import _lib
-from ._lib import (ACT_GELU_ERF, ACT_GELU_TANH, ACT_NONE, ACT_QUICK_GELU, ACT_SILU, OUT_BF16, OUT_F32,
+from ._lib import (ACT_GELU_ERF, ACT_GELU_TANH, ACT_NONE, ACT_QUICK_GELU, ACT_SILU, OUT_BF16, OUT_F32, OUT_FP8,
                    OUT_RESID_F32)
 
-__all__ = ["gemm", "ACT_NONE", "ACT_GELU_ERF", "ACT_GELU_TANH", "ACT_SILU", "ACT_QUICK_GELU", "OUT_BF16", "OUT_F32",
-           "OUT_RESID_F32"]
+__all__ = ["gemm", "gemm_fp8", "norm_modulate_fp8", "quantize_fp8", "quantize_weight_fp8", "ACT_NONE", "ACT_GELU_ERF",
+           "ACT_GELU_TANH", "ACT_SILU", "ACT_QUICK_GELU", "OUT_BF16", "OUT_F32", "OUT_RESID_F32", "OUT_FP8"]
+
+FP8 = torch.float8_e4m3fn
+FP8_MAX = 448.0
 
 
 def _req(cond: bool, msg: str) -> None:
@@ -148,6 +151,19 @@ def norm_modulate(x: torch.Tensor, *, norm: int, shift: torch.Tensor | None = No
     else:
         _req(resid is not None, "want_out=False needs a residual update")
         out = None
+    _norm_modulate_inputs(a, x, norm=norm, shift=shift, scale=scale, mod_rows=mod_rows, shift_tab=shift_tab,
+                          scale_tab=scale_tab, weight=weight, eps=eps, act=act, resid=resid, resid_gate=resid_gate,
+                          resid_gate_rows=resid_gate_rows, resid_bcast=resid_bcast, resid_bcast_rows=resid_bcast_rows,
+                          resid_rows=resid_rows, resid_out_gate=resid_out_gate, resid_out_gate_rows=resid_out_gate_rows)
+    _lib.check(_lib.lib().ln3_norm_modulate(C.byref(a), _lib.current_stream()), "ln3_norm_modulate")
+    return out
+
+
+def _norm_modulate_inputs(a, x, *, norm, shift, scale, mod_rows, shift_tab, scale_tab, weight, eps, act, resid,
+                          resid_gate, resid_gate_rows, resid_bcast, resid_bcast_rows, resid_rows, resid_out_gate,
+                          resid_out_gate_rows) -> None:
+    """Checks every input of norm_modulate except the output and fills them into the NormModulateArgs `a`."""
+    rows, D = x.shape
     if resid is not None:
         _cuda(resid, "resid", torch.bfloat16)
         _req(resid.shape == (rows, D) and resid.stride(1) == 1, "resid must be (rows, D) bf16")
@@ -194,8 +210,124 @@ def norm_modulate(x: torch.Tensor, *, norm: int, shift: torch.Tensor | None = No
         _req(weight.shape == (D,) and weight.is_contiguous(), "weight must be contiguous (D,)")
         a.weight = weight.data_ptr()
     a.norm, a.act, a.eps = norm, act, eps
-    _lib.check(_lib.lib().ln3_norm_modulate(C.byref(a), _lib.current_stream()), "ln3_norm_modulate")
-    return out
+
+
+def _fp8_pair(rows: int, cols: int, device, out, out_scale, what: str):
+    """Checked (or new) e4m3 codes (rows, cols) and fp32 block scales (rows, cols/128) with unit inner strides."""
+    if out is None:
+        out = torch.empty((rows, cols), device=device, dtype=FP8)
+    if out_scale is None:
+        out_scale = torch.empty((rows, cols // 128), device=device, dtype=torch.float32)
+    _cuda(out, f"{what} out", FP8)
+    _cuda(out_scale, f"{what} out_scale", torch.float32)
+    _req(out.shape == (rows, cols) and out.stride(1) == 1, f"{what}: out must be ({rows}, {cols}) with unit inner stride")
+    _req(out_scale.shape == (rows, cols // 128) and out_scale.stride(1) == 1,
+         f"{what}: out_scale must be ({rows}, {cols // 128}) with unit inner stride")
+    return out, out_scale
+
+
+def norm_modulate_fp8(x: torch.Tensor, *, norm: int, out: torch.Tensor | None = None,
+                      out_scale: torch.Tensor | None = None, shift: torch.Tensor | None = None,
+                      scale: torch.Tensor | None = None, mod_rows: int = 1,
+                      shift_tab: torch.Tensor | None = None, scale_tab: torch.Tensor | None = None,
+                      weight: torch.Tensor | None = None, eps: float = 1e-6, act: int = ACT_NONE,
+                      resid: torch.Tensor | None = None, resid_gate: torch.Tensor | None = None,
+                      resid_gate_rows: int = 1, resid_bcast: torch.Tensor | None = None, resid_bcast_rows: int = 1,
+                      resid_rows: tuple | None = None, resid_out_gate: torch.Tensor | None = None,
+                      resid_out_gate_rows: int = 1):
+    """norm_modulate with an fp8 output: returns (codes e4m3 (rows, D), block scales fp32 (rows, D/128)) in the
+    1 x 128 block format of include/ln3b200.h.  The residual update of x is the bf16 op's, bit for bit."""
+    _cuda(x, "x", torch.float32)
+    _req(x.dim() == 2 and x.stride(1) == 1, "x must be (rows, D) with unit inner stride")
+    rows, D = x.shape
+    _req(D % 128 == 0, f"D={D} must be a multiple of 128")
+    out, out_scale = _fp8_pair(rows, D, x.device, out, out_scale, "norm_modulate_fp8")
+    f = _lib.NormModulateFp8Args()
+    _norm_modulate_inputs(f.base, x, norm=norm, shift=shift, scale=scale, mod_rows=mod_rows, shift_tab=shift_tab,
+                          scale_tab=scale_tab, weight=weight, eps=eps, act=act, resid=resid, resid_gate=resid_gate,
+                          resid_gate_rows=resid_gate_rows, resid_bcast=resid_bcast, resid_bcast_rows=resid_bcast_rows,
+                          resid_rows=resid_rows, resid_out_gate=resid_out_gate, resid_out_gate_rows=resid_out_gate_rows)
+    f.out, f.ldo = out.data_ptr(), out.stride(0)
+    f.out_scale, f.out_scale_ld = out_scale.data_ptr(), out_scale.stride(0)
+    _lib.check(_lib.lib().ln3_norm_modulate_fp8(C.byref(f), _lib.current_stream()), "ln3_norm_modulate_fp8")
+    return out, out_scale
+
+
+def quantize_fp8(x: torch.Tensor, out: torch.Tensor | None = None, out_scale: torch.Tensor | None = None):
+    """x fp32 or bf16 (rows, D), D % 128 == 0 -> (e4m3 codes (rows, D), fp32 block scales (rows, D/128)):
+    s = fp32(absmax of the 128-column block / 448), code = e4m3 rn-satfinite of fp32(x / s); s = 0 -> zero codes."""
+    _cuda(x, "x")
+    _req(x.dtype in (torch.float32, torch.bfloat16), f"x must be float32 or bfloat16, got {x.dtype}")
+    _req(x.dim() == 2 and x.stride(1) == 1, "x must be (rows, D) with unit inner stride")
+    rows, D = x.shape
+    _req(D > 0 and D % 128 == 0, f"D={D} must be a positive multiple of 128")
+    out, out_scale = _fp8_pair(rows, D, x.device, out, out_scale, "quantize_fp8")
+    _lib.check(_lib.lib().ln3_quantize_fp8_rows(
+        x.data_ptr(), int(x.dtype == torch.bfloat16), x.stride(0), rows, D, out.data_ptr(), out.stride(0),
+        out_scale.data_ptr(), out_scale.stride(0), _lib.current_stream()), "ln3_quantize_fp8_rows")
+    return out, out_scale
+
+
+@torch.no_grad()
+def quantize_weight_fp8(w: torch.Tensor):
+    """nn.Linear weight (N, K) -> (e4m3 codes (N, K), fp32 per-output-channel scales (N,)), on w's device:
+    w_scale = fp32(absmax of the row / 448), codes = torch's float8_e4m3fn cast of fp32(w / w_scale); a zero row has
+    scale 0 and zero codes.  Runs once per model (prepare()), not on the hot path."""
+    w = w.detach().float()
+    amax = w.abs().amax(dim=1)
+    s = amax / torch.full_like(amax, FP8_MAX)     # elementwise division (a Python scalar divisor becomes * (1/448))
+    q = torch.where(s[:, None] > 0, w / torch.where(s > 0, s, torch.ones_like(s))[:, None], torch.zeros_like(w))
+    return q.clamp(-FP8_MAX, FP8_MAX).to(FP8).contiguous(), s.contiguous()
+
+
+def gemm_fp8(a_q: torch.Tensor, a_scale: torch.Tensor, w_q: torch.Tensor, w_scale: torch.Tensor,
+             bias: torch.Tensor | None = None, *, act: int = ACT_NONE, out_kind: int = OUT_BF16,
+             out: torch.Tensor | None = None, out_scale: torch.Tensor | None = None,
+             head_norm: torch.Tensor | None = None, head_norm_sec_cols: int = 0, head_norm_eps: float = 1e-5):
+    """out = epilogue(w_scale[n] * sum_kb a_scale[m, kb] * (a_q[m, kb] . w_q[n, kb])) on the fp8 tensor cores.
+    a_q (M, K) and w_q (N, K) e4m3 codes, a_scale (M, K/128) and w_scale (N,) fp32 (format: include/ln3b200.h).
+    OUT_BF16 (act NONE, optional head_norm as in `gemm`) returns the bf16 (M, N) output; OUT_FP8 (act NONE or
+    GELU_ERF) returns (codes (M, N), block scales (M, N/128)), the A operand of a following gemm_fp8."""
+    _cuda(a_q, "a_q", FP8)
+    _cuda(w_q, "w_q", FP8)
+    _cuda(a_scale, "a_scale", torch.float32)
+    _cuda(w_scale, "w_scale", torch.float32)
+    _req(a_q.dim() == 2 and w_q.dim() == 2, "a_q and w_q must be 2-D")
+    _req(a_q.stride(1) == 1 and w_q.stride(1) == 1, "a_q and w_q must have unit inner stride")
+    M, K = a_q.shape
+    N, K2 = w_q.shape
+    _req(K == K2, f"inner dims differ: {K} vs {K2}")
+    _req(K % 128 == 0 and N % 128 == 0, f"K={K} and N={N} must be multiples of 128")
+    _req(a_scale.dim() == 2 and a_scale.shape == (M, K // 128) and a_scale.stride(1) == 1,
+         f"a_scale must be ({M}, {K // 128}) with unit inner stride")
+    _req(w_scale.shape == (N,) and w_scale.is_contiguous(), f"w_scale must be contiguous ({N},)")
+    args = _lib.GemmFp8Args()
+    if out_kind == OUT_FP8:
+        out, out_scale = _fp8_pair(M, N, a_q.device, out, out_scale, "gemm_fp8")
+        args.out_scale, args.out_scale_ld = out_scale.data_ptr(), out_scale.stride(0)
+    else:
+        _req(out_kind == OUT_BF16, "gemm_fp8 writes OUT_BF16 or OUT_FP8")
+        if out is None:
+            out = torch.empty((M, N), device=a_q.device, dtype=torch.bfloat16)
+        _cuda(out, "out", torch.bfloat16)
+        _req(out.shape == (M, N) and out.stride(1) == 1, "out must be (M,N) with unit inner stride")
+    args.A, args.a_scale, args.W, args.w_scale = a_q.data_ptr(), a_scale.data_ptr(), w_q.data_ptr(), w_scale.data_ptr()
+    args.out = out.data_ptr()
+    args.M, args.N, args.K = M, N, K
+    args.lda, args.ldw, args.ldo, args.a_scale_ld = a_q.stride(0), w_q.stride(0), out.stride(0), a_scale.stride(0)
+    if bias is not None:
+        _cuda(bias, "bias", torch.float32)
+        _req(bias.shape == (N,) and bias.is_contiguous(), "bias must be contiguous (N,)")
+        args.bias = bias.data_ptr()
+    if head_norm is not None:
+        _cuda(head_norm, "head_norm", torch.float32)
+        _req(head_norm.dim() == 2 and head_norm.shape[1] == 64 and head_norm.is_contiguous(),
+             "head_norm must be contiguous (nsec, 64)")
+        args.head_norm_w, args.head_norm_nsec = head_norm.data_ptr(), head_norm.shape[0]
+        args.head_norm_sec_cols, args.head_norm_eps = head_norm_sec_cols, head_norm_eps
+    args.act, args.out_kind = act, out_kind
+    _lib.check(_lib.lib().ln3_gemm_fp8(C.byref(args), _lib.current_stream()), "ln3_gemm_fp8")
+    return (out, out_scale) if out_kind == OUT_FP8 else out
 
 
 def timestep_embedding(t: torch.Tensor, out: torch.Tensor | None = None) -> torch.Tensor:
