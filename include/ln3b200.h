@@ -283,6 +283,44 @@ typedef struct ln3_sampler_update_args {
 
 int ln3_sampler_affine_update(const ln3_sampler_update_args* args, void* stream);
 
+/* ------------------------------------------------------------------ fused sampler step (sgm sampler family)
+ * The elementwise tail of one denoiser evaluation of every sgm EDM-family sampler, per element of sample b
+ * (all scalars per sample, coef row b = (k0, k1, k2, a, b, c, h0, h1, h2, s, 0, 0), [B, 12] fp32):
+ *   e = k0 * x_eval + k1 * net_u + k2 * net_c        the guided denoised D, or the derivative d
+ *   v = a * x + b * x_eval + c * e + h0 * hist[0] + h1 * hist[1] + h2 * hist[2] + s * noise
+ *   x_out[b] = v;  eval_out[b] = eval_out[B + b] = v (both halves of the next 2B CFG input);  hist_out[b] = e
+ * evaluated left to right as one fmaf chain.  net_u / net_c are the network's uncond / cond output halves
+ * (EpsScaling: D = x_eval - sigma_q * net); net_c is NULL for IdentityGuider; a NULL hist[j] or noise drops its
+ * term; a NULL output is not written.  Covers:
+ *   VanillaCFG / IdentityGuider + DiscreteDenoiser(EpsScaling)   guiders.py:24-42, denoiser.py:25-42,
+ *       denoiser_scaling.py:29-37
+ *   EulerAncestralSampler    sampling.py:133-170,237-244 (ancestral Euler + noise), sampling_utils.py:22-35
+ *   HeunEDMSampler           sampling.py:93-107,218-234 (predictor writes x_euler + d, corrector averages)
+ *   DPMPP2SAncestralSampler  sampling.py:247-284, sampling_utils.py:38-43 (midpoint evaluation, mult1..4)
+ *   DPMPP2MSampler           sampling.py:287-362 (previous guided D in hist[0])
+ *   LinearMultistepSampler   sampling.py:173-208, sampling_utils.py:7-19 (up to 3 past derivatives)
+ * n_per_sample % 4 == 0; every non-NULL pointer 16-byte aligned; x, x_eval, net_u and coef non-NULL; at least one
+ * output.  x_eval, net_*, hist[j], noise and x_out hold B rows, eval_out 2B rows.  No output may overlap another
+ * output or an input, except x_out == x and eval_out == x_eval (same start: the element is read before it is
+ * written by the same thread).  LN3_EINVAL otherwise, before any CUDA call.
+ */
+typedef struct ln3_sampler_step_args {
+  const float* x;
+  const float* x_eval;
+  const float* net_u;
+  const float* net_c;
+  const float* hist[3];
+  const float* noise;
+  const float* coef;
+  float* x_out;
+  float* eval_out;
+  float* hist_out;
+  int B;
+  long long n_per_sample;
+} ln3_sampler_step_args;
+
+int ln3_sampler_step(const ln3_sampler_step_args* args, void* stream);
+
 /* ------------------------------------------------------------------ grouped adaptive dopri5
  * The per-attempt arithmetic of the adaptive Dormand-Prince 5(4) solver that `sample_ode`'s default runs
  * (transport/transport.py:374-421 -> transport/integrators.py:101-120 -> torchdiffeq odeint(method='dopri5')),

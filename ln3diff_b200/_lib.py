@@ -116,6 +116,15 @@ class SamplerUpdateArgs(C.Structure):
     ]
 
 
+class SamplerStepArgs(C.Structure):
+    _fields_ = [
+        ("x", C.c_void_p), ("x_eval", C.c_void_p), ("net_u", C.c_void_p), ("net_c", C.c_void_p),
+        ("hist", C.c_void_p * 3), ("noise", C.c_void_p), ("coef", C.c_void_p),
+        ("x_out", C.c_void_p), ("eval_out", C.c_void_p), ("hist_out", C.c_void_p),
+        ("B", C.c_int), ("n_per_sample", C.c_longlong),
+    ]
+
+
 class RenderArgs(C.Structure):
     _fields_ = [
         ("planes_cl", C.c_void_p), ("view_obj", C.c_void_p), ("ray_o", C.c_void_p),

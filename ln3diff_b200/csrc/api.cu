@@ -167,6 +167,46 @@ static int ode_validate(const ln3_ode_args* a, int need, const char* what) {
   return LN3_OK;
 }
 
+// The rules of ln3_sampler_step (include/ln3b200.h): shapes, NULLs, alignment, and no output range overlapping
+// another output or an input except the two in-place aliases x_out == x and eval_out == x_eval.
+static int sampler_step_validate(const ln3_sampler_step_args* a) {
+  if (!a) return set_error(LN3_EINVAL, "sampler_step: null args");
+  if (a->B < 0 || a->n_per_sample < 0) return set_error(LN3_EINVAL, "sampler_step: negative B or n_per_sample");
+  if (a->n_per_sample % 4) return set_error(LN3_EINVAL, "sampler_step: n_per_sample % 4 != 0");
+  if (a->B > 0 && a->n_per_sample > (1ll << 50) / (8ll * a->B))
+    return set_error(LN3_EINVAL, "sampler_step: B * n_per_sample too large");
+  if (!a->x || !a->x_eval || !a->net_u || !a->coef)
+    return set_error(LN3_EINVAL, "sampler_step: null x, x_eval, net_u or coef");
+  if (!a->x_out && !a->eval_out && !a->hist_out) return set_error(LN3_EINVAL, "sampler_step: no output");
+  struct Range { const char* name; const void* p; unsigned long long bytes; };
+  const unsigned long long row = 4ull * static_cast<unsigned long long>(a->B) * a->n_per_sample;
+  const Range in[] = {{"x", a->x, row}, {"x_eval", a->x_eval, row}, {"net_u", a->net_u, row},
+                      {"net_c", a->net_c, row}, {"hist[0]", a->hist[0], row}, {"hist[1]", a->hist[1], row},
+                      {"hist[2]", a->hist[2], row}, {"noise", a->noise, row},
+                      {"coef", a->coef, 48ull * static_cast<unsigned long long>(a->B)}};
+  const Range out[] = {{"x_out", a->x_out, row}, {"eval_out", a->eval_out, 2 * row}, {"hist_out", a->hist_out, row}};
+  for (const Range& r : in)
+    if (misaligned16(r.p)) return set_error(LN3_EINVAL, "sampler_step: %s must be 16-byte aligned", r.name);
+  for (const Range& r : out)
+    if (misaligned16(r.p)) return set_error(LN3_EINVAL, "sampler_step: %s must be 16-byte aligned", r.name);
+  auto overlap = [](const Range& u, const Range& v) {
+    if (!u.p || !v.p || u.bytes == 0 || v.bytes == 0) return false;
+    const uintptr_t a0 = reinterpret_cast<uintptr_t>(u.p), b0 = reinterpret_cast<uintptr_t>(v.p);
+    return a0 < b0 + v.bytes && b0 < a0 + u.bytes;
+  };
+  for (int i = 0; i < 3; ++i) {
+    for (int j = i + 1; j < 3; ++j)
+      if (overlap(out[i], out[j]))
+        return set_error(LN3_EINVAL, "sampler_step: outputs %s and %s overlap", out[i].name, out[j].name);
+    for (int j = 0; j < 9; ++j) {
+      const bool alias = out[i].p == in[j].p && ((i == 0 && j == 0) || (i == 1 && j == 1));
+      if (!alias && overlap(out[i], in[j]))
+        return set_error(LN3_EINVAL, "sampler_step: output %s overlaps input %s", out[i].name, in[j].name);
+    }
+  }
+  return LN3_OK;
+}
+
 }  // namespace ln3
 
 using namespace ln3;
@@ -211,6 +251,11 @@ int ln3_final_layer(const ln3_final_layer_args* args, void* stream) {
 int ln3_sampler_affine_update(const ln3_sampler_update_args* args, void* stream) {
   if (!args) return set_error(LN3_EINVAL, "sampler_update: null args");
   return sampler_affine_update(args, static_cast<cudaStream_t>(stream));
+}
+int ln3_sampler_step(const ln3_sampler_step_args* args, void* stream) {
+  const int rc = sampler_step_validate(args);
+  if (rc != LN3_OK) return rc;
+  return sampler_step(args, static_cast<cudaStream_t>(stream));
 }
 
 size_t ln3_render_workspace_bytes(int V, int M, int group_size) {

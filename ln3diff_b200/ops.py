@@ -470,6 +470,65 @@ def sampler_affine_update(x: torch.Tensor, coef: torch.Tensor, m0: torch.Tensor,
     return out
 
 
+SAMPLER_STEP_COEFS = 12   # (k0, k1, k2, a, b, c, h0, h1, h2, s, 0, 0)
+
+
+def sampler_step(x: torch.Tensor, x_eval: torch.Tensor, coef: torch.Tensor, net_u: torch.Tensor,
+                 net_c: torch.Tensor | None = None, hist=(), noise: torch.Tensor | None = None, *,
+                 x_out: torch.Tensor | None = None, eval_out: torch.Tensor | None = None,
+                 hist_out: torch.Tensor | None = None) -> None:
+    """One sampler evaluation's elementwise tail (include/ln3b200.h, ln3_sampler_step_args), per sample b:
+        e = k0 x_eval + k1 net_u + k2 net_c
+        v = a x + b x_eval + c e + h0 hist[0] + h1 hist[1] + h2 hist[2] + s noise
+        x_out[b] = v;  eval_out[b] = eval_out[B+b] = v;  hist_out[b] = e
+    coef (B, 12) fp32.  Every tensor is CUDA fp32, contiguous and 16-byte aligned, with B rows of n elements
+    (n % 4 == 0) except eval_out's 2B.  Outputs are written in place; at least one is required.  No output may
+    overlap another output or an input, except x_out is x and eval_out starting at x_eval."""
+    _cuda(x, "x", torch.float32)
+    B = x.shape[0]
+    n = x[0].numel() if B else 0
+    _cuda(coef, "coef", torch.float32)
+    _req(coef.shape == (B, SAMPLER_STEP_COEFS) and coef.is_contiguous(), "coef must be contiguous (B, 12)")
+    hist = tuple(hist)
+    _req(len(hist) <= 3, "at most 3 history operands")
+    hist = hist + (None,) * (3 - len(hist))
+    ins = [("x", x), ("x_eval", x_eval), ("net_u", net_u), ("net_c", net_c), ("hist[0]", hist[0]),
+           ("hist[1]", hist[1]), ("hist[2]", hist[2]), ("noise", noise)]
+    outs = [("x_out", x_out, B), ("eval_out", eval_out, 2 * B), ("hist_out", hist_out, B)]
+    _req(x_eval is not None and net_u is not None, "x_eval and net_u are required")
+    _req(any(t_ is not None for _, t_, _ in outs), "at least one of x_out, eval_out, hist_out is required")
+    _req(n % 4 == 0, "elements per sample must be a multiple of 4")
+    for nm, t_, rows in [(nm, t_, B) for nm, t_ in ins] + outs:
+        if t_ is None:
+            continue
+        _cuda(t_, nm, torch.float32)
+        _req(t_.is_contiguous() and t_.shape[0] == rows and t_.numel() == rows * n,
+             f"{nm} must be contiguous with {rows} rows of {n} elements")
+        _req(t_.data_ptr() % 16 == 0, f"{nm} must be 16-byte aligned (the kernel uses 128-bit accesses)")
+    _req(coef.data_ptr() % 16 == 0, "coef must be 16-byte aligned")
+
+    def span(t_):
+        return t_.data_ptr(), t_.data_ptr() + t_.numel() * 4
+
+    in_spans = [(nm, t_) for nm, t_ in ins if t_ is not None] + [("coef", coef)]
+    out_spans = [(nm, t_) for nm, t_, _ in outs if t_ is not None]
+    for i, (on, ot) in enumerate(out_spans):
+        o0, o1 = span(ot)
+        for nm, t_ in out_spans[i + 1:] + in_spans:
+            a0, a1 = span(t_)
+            alias = ot.data_ptr() == t_.data_ptr() and (on, nm) in (("x_out", "x"), ("eval_out", "x_eval"))
+            _req(alias or o1 <= a0 or a1 <= o0, f"{on} overlaps {nm}")
+    a = _lib.SamplerStepArgs()
+    a.x, a.x_eval, a.net_u, a.coef = x.data_ptr(), x_eval.data_ptr(), net_u.data_ptr(), coef.data_ptr()
+    ptr = lambda t_: t_.data_ptr() if t_ is not None else None
+    a.net_c, a.noise = ptr(net_c), ptr(noise)
+    for j in range(3):
+        a.hist[j] = ptr(hist[j])
+    a.x_out, a.eval_out, a.hist_out = ptr(x_out), ptr(eval_out), ptr(hist_out)
+    a.B, a.n_per_sample = B, n
+    _lib.check(_lib.lib().ln3_sampler_step(C.byref(a), _lib.current_stream()), "ln3_sampler_step")
+
+
 # ---------------------------------------------------------------------------------------------- grouped dopri5
 ODE_GROUP_BYTES = C.sizeof(_lib.OdeGroup)
 _ODE_F64 = ("t", "dt", "t_prev", "dt_step", "ratio", "aux")

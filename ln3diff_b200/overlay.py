@@ -36,6 +36,7 @@ MIRRORED = {
     "dit.dit_decoder": "ln3diff_b200.dit.dit_decoder",
     "dit.dit_models_xformers": "ln3diff_b200.dit.dit_models_xformers",
     "sgm.modules.diffusionmodules.sampling": "ln3diff_b200.sgm.modules.diffusionmodules.sampling",
+    "sgm.modules.diffusionmodules.sampling_utils": "ln3diff_b200.sgm.modules.diffusionmodules.sampling_utils",
     "sgm.modules.diffusionmodules.denoiser": "ln3diff_b200.sgm.modules.diffusionmodules.denoiser",
     "sgm.modules.diffusionmodules.denoiser_scaling": "ln3diff_b200.sgm.modules.diffusionmodules.denoiser_scaling",
     "sgm.modules.diffusionmodules.discretizer": "ln3diff_b200.sgm.modules.diffusionmodules.discretizer",

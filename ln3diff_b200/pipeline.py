@@ -45,14 +45,194 @@ def edm_cfg_tables(num_steps: int, scale: float, B: int, device, dtype=torch.flo
     )
 
 
+# ---------------------------------------------------------------------------------------------- sgm sampler family
+# The reference's class names (sgm/inference/api.py:30-34) of the samplers sample_t23d runs.
+SAMPLERS = ("EulerEDMSampler", "HeunEDMSampler", "EulerAncestralSampler", "DPMPP2SAncestralSampler",
+            "DPMPP2MSampler", "LinearMultistepSampler")
+_PLANS: dict = {}
+
+
+def _plan_eval(plan, step, sigma, coef, *, kind, hist=(), hist_write=None, noise=False, draw=False, x_out=True):
+    """Append one denoiser evaluation at `sigma` (a float32 scalar tensor).  kind 'D': e is the guided denoised D;
+    kind 'd': e is the derivative (x_eval - D) / sigma.  coef holds the update part (a, b, c, h0, h1, h2, s)."""
+    table = plan["_table"]
+    idx = (sigma - table).abs().argmin()                          # DiscreteDenoiser.sigma_to_idx
+    sq = table[idx]                                               # possibly_quantize_sigma
+    idx2 = (sq - table).abs().argmin()                            # possibly_quantize_c_noise
+    c_in = 1 / (sq ** 2 + 1.0) ** 0.5                             # EpsScaling
+    g, sqd = plan["scale"], float(sq)
+    if kind == "D":                                               # D = x_eval - sq net, CFG-combined
+        k = (1.0, -sqd * (1 - g), -sqd * g)
+    else:                                                         # d = (x_eval - D) / sigma = sq net / sigma
+        k = (0.0, sqd * (1 - g) / float(sigma), sqd * g / float(sigma))
+    row = list(k) + [float(coef.get(n, 0.0)) for n in ("a", "b", "c", "h0", "h1", "h2", "s")] + [0.0, 0.0]
+    plan["evals"].append(dict(step=step, sigma=float(sigma), t_idx=int(idx2), c_in=float(c_in), coef=row,
+                              hist=tuple(hist), hist_write=hist_write, noise=noise, draw=draw, x_out=x_out,
+                              eval_out=True))
+
+
+def edm_sampler_plan(sampler: str, num_steps: int, scale: float, eta: float = 1.0, s_noise: float = 1.0,
+                     order: int = 4) -> dict:
+    """The evaluation plan of one sgm sampler run with DiscreteDenoiser(EpsScaling, 1000) + VanillaCFG(scale) on
+    the LegacyDDPM schedule (host-side, float32 scalar ops in the reference's order; cached).  One entry per
+    denoiser evaluation: its sigma, timestep index and c_in, the ln3_sampler_step coefficient row
+    (k0, k1, k2, a, b, c, h0, h1, h2, s, 0, 0) for the raw network halves, the history slots it reads (hist[j])
+    and writes, whether it reads the step's noise / draws it, and which of x and the next forward's input it
+    writes.  Reference: sgm/modules/diffusionmodules/sampling.py:133-362, sampling_utils.py:7-43."""
+    from .sgm.modules.diffusionmodules.sampling_utils import get_ancestral_step, linear_multistep_coeff
+    if sampler not in SAMPLERS[1:]:
+        raise ValueError(f"unknown sampler {sampler!r}; expected one of {SAMPLERS}")
+    if sampler == "LinearMultistepSampler" and not 1 <= order <= 4:
+        raise ValueError("LinearMultistepSampler: the fused step keeps at most 3 past derivatives (order <= 4)")
+    key = (sampler, int(num_steps), float(scale), float(eta), float(s_noise), int(order))
+    plan = _PLANS.get(key)
+    if plan is not None:
+        return plan
+    disc = LegacyDDPMDiscretization()
+    sig = disc(num_steps, device="cpu")                           # (num_steps+1,) float32, last = 0
+    plan = dict(sampler=sampler, num_steps=num_steps, scale=scale, evals=[], sigmas=sig, n_slots=0,
+                init_scale=float(torch.sqrt(1.0 + sig[0] ** 2.0)),
+                _table=disc(1000, do_append_zero=False, flip=True))
+    ancestral = sampler in ("EulerAncestralSampler", "DPMPP2SAncestralSampler")
+    nlog = lambda s: s.log().neg()                                # to_neg_log_sigma
+    tsig = lambda t: t.neg().exp()                                # to_sigma
+    sig_np = sig.numpy()
+    for i in range(num_steps):
+        s, sn = sig[i], sig[i + 1]
+        if ancestral:
+            sd, su = get_ancestral_step(s, sn, eta=eta)
+            su = torch.as_tensor(su, dtype=torch.float32)
+            # ancestral_step: x + noise * s_noise * sigma_up where next_sigma > 0 (one draw per step regardless)
+            ns = dict(s=float(s_noise * su) if float(sn) > 0.0 else 0.0)
+            nread = float(sn) > 0.0
+        if sampler == "EulerAncestralSampler":
+            r = (sd - s) / s                                      # x + (sd - s) (x - D) / s
+            _plan_eval(plan, i, s, dict(a=1 + r, c=-r, **ns), kind="D", noise=nread, draw=True)
+        elif sampler == "DPMPP2SAncestralSampler":
+            if float(sd) < 1e-14:
+                r = (sd - s) / s
+                _plan_eval(plan, i, s, dict(a=1 + r, c=-r, **ns), kind="D", noise=nread, draw=True)
+            else:
+                t, tn = nlog(s), nlog(sd)
+                h = tn - t
+                sm = t + 0.5 * h
+                m1, m2 = tsig(sm) / tsig(t), (-0.5 * h).expm1()
+                m3, m4 = tsig(tn) / tsig(t), (-h).expm1()
+                _plan_eval(plan, i, s, dict(a=m1, c=-m2), kind="D", x_out=False)           # x2 -> next input
+                _plan_eval(plan, i, tsig(sm), dict(a=m3, c=-m4, **ns), kind="D", noise=nread, draw=True)
+        elif sampler == "HeunEDMSampler":
+            dt = sn - s
+            if float(sn) < 1e-14:
+                _plan_eval(plan, i, s, dict(a=1.0, c=dt), kind="d")
+            else:
+                plan["n_slots"] = 1
+                _plan_eval(plan, i, s, dict(a=1.0, c=dt), kind="d", hist_write=0, x_out=False)   # x_euler, d
+                _plan_eval(plan, i, sn, dict(a=1.0, c=dt / 2.0, h0=dt / 2.0), kind="d", hist=(0,))
+        elif sampler == "DPMPP2MSampler":
+            t, tn = nlog(s), nlog(sn)
+            h = tn - t
+            m1, m2 = tsig(tn) / tsig(t), (-h).expm1()
+            plan["n_slots"] = 2
+            if i == 0 or float(sn) < 1e-14:
+                _plan_eval(plan, i, s, dict(a=m1, c=-m2), kind="D", hist_write=i % 2)
+            else:
+                rr = (t - nlog(sig[i - 1])) / h
+                m3, m4 = 1 + 1 / (2 * rr), 1 / (2 * rr)
+                _plan_eval(plan, i, s, dict(a=m1, c=-float(m2) * float(m3), h0=float(m2) * float(m4)), kind="D",
+                           hist=((i - 1) % 2,), hist_write=i % 2)
+        else:                                                     # LinearMultistepSampler
+            cur = min(i + 1, order)
+            cf = [linear_multistep_coeff(cur, sig_np, i, j) for j in range(cur)]
+            plan["n_slots"] = order
+            hist = tuple((i - 1 - j) % order for j in range(cur - 1))
+            _plan_eval(plan, i, s, dict(a=1.0, c=cf[0], **{f"h{j}": cf[j + 1] for j in range(cur - 1)}), kind="d",
+                       hist=hist, hist_write=i % order)
+    plan["evals"][-1]["eval_out"] = False                         # nothing reads the input after the last forward
+    if plan["evals"][-1]["hist_write"] is not None:
+        plan["evals"][-1]["hist_write"] = None
+    E = len(plan["evals"])
+    plan["coef"] = torch.tensor([e["coef"] for e in plan["evals"]], dtype=torch.float32).reshape(E, 12)
+    plan["t_idx"] = torch.tensor([float(e["t_idx"]) for e in plan["evals"]], dtype=torch.float32)
+    plan["c_in"] = torch.tensor([e["c_in"] for e in plan["evals"]], dtype=torch.float32)
+    del plan["_table"]
+    _PLANS[key] = plan
+    return plan
+
+
+@torch.no_grad()
+def _sample_t23d_plan(model, randn, c, uc, plan, use_graph, noise):
+    """The evaluation plan's loop: one DiT forward of the 2B CFG batch per entry (a graph replay), then one
+    ln3_sampler_step that writes the state, both halves of the next forward's input and the history slot."""
+    B, dev = randn.shape[0], randn.device
+    E = len(plan["evals"])
+    if noise is not None and (tuple(noise.shape) != (plan["num_steps"],) + tuple(randn.shape) or not noise.is_cuda):
+        raise ValueError(f"noise must be a CUDA tensor of shape {(plan['num_steps'],) + tuple(randn.shape)}")
+    tabs = plan.setdefault("_device", {}).get((B, dev))
+    if tabs is None:
+        tabs = plan["_device"][(B, dev)] = dict(
+            t_idx=plan["t_idx"].to(dev)[:, None].repeat(1, 2 * B).contiguous(),
+            c_in=plan["c_in"].to(dev)[:, None].repeat(1, 2 * B).contiguous(),
+            coef=plan["coef"].to(dev)[:, None, :].repeat(1, B, 1).contiguous())
+    ctx = torch.cat((uc["crossattn"], c["crossattn"]), 0).contiguous()   # VanillaCFG order: (uc, c)
+    xs = (randn.float() * plan["init_scale"]).contiguous()
+    slots = [torch.empty_like(xs) for _ in range(plan["n_slots"])]
+    graph = use_graph and graphs_enabled() and hasattr(model, "capture_graph")
+    if graph:
+        shared = hasattr(model, "modulation_table") and os.environ.get("LN3_SHARED_MODULATION", "1") != "0"
+        g = model.capture_graph(2 * B, ctx, shared_mod=shared)
+        mod_table = model.modulation_table(tabs["t_idx"][:, 0]) if shared else None
+        xin = g.x
+    else:
+        xin = torch.empty((2 * B,) + tuple(xs.shape[1:]), device=dev, dtype=torch.float32)
+    xin[:B].copy_(xs)
+    xin[B:].copy_(xs)
+    for k, ev in enumerate(plan["evals"]):
+        if graph:
+            if shared:
+                g.mod.copy_(mod_table[k:k + 1])
+            else:
+                g.t.copy_(tabs["t_idx"][k])
+            g.in_scale.copy_(tabs["c_in"][k])
+            g.replay()
+            net = g.out
+        else:
+            net = model(xin, tabs["t_idx"][k], ctx, in_scale=tabs["c_in"][k])
+        nz = None
+        if ev["draw"]:
+            nz = noise[ev["step"]] if noise is not None else torch.randn_like(xs)
+        ops.sampler_step(xs, xin[:B], tabs["coef"][k], net[:B], net[B:], [slots[j] for j in ev["hist"]],
+                         nz if ev["noise"] else None, x_out=xs if ev["x_out"] else None,
+                         eval_out=xin if ev["eval_out"] else None,
+                         hist_out=slots[ev["hist_write"]] if ev["hist_write"] is not None else None)
+    return xs
+
+
 @torch.no_grad()
 def sample_t23d(model, randn: torch.Tensor, c: dict, uc: dict, num_steps: int = 250,
-                scale: float = 6.5, tables: dict | None = None, use_graph: bool = True) -> torch.Tensor:
+                scale: float = 6.5, tables: dict | None = None, use_graph: bool = True,
+                sampler: str = "EulerEDMSampler", eta: float = 1.0, s_noise: float = 1.0, order: int = 4,
+                noise: torch.Tensor | None = None, s_churn: float = 0.0) -> torch.Tensor:
     """randn (B, 12, 32, 32) fp32 on the GPU (the reference draws it on the CPU generator and moves
     it, sgm_DiffusionEngine.py:395); c / uc = {'crossattn': (B, 77, ctx_dim)}.  Returns the
-    denoised latents (B, 12, 32, 32) fp32."""
+    denoised latents (B, 12, 32, 32) fp32.
+
+    `sampler` is one of the reference's sgm class names (SAMPLERS): 'EulerEDMSampler' (the default, the
+    engine's) or HeunEDMSampler, EulerAncestralSampler, DPMPP2SAncestralSampler, DPMPP2MSampler and
+    LinearMultistepSampler with the reference's parameters eta / s_noise (ancestral), order (LMS).  The ancestral
+    samplers draw one `torch.randn_like` of the state per step on the device generator, in the reference's order;
+    `noise` (num_steps, B, 12, 32, 32) replaces those draws.  `tables` (edm_cfg_tables) is Euler-only.  Stochastic
+    churn (s_churn > 0) is not fused: use the mirrored sampler classes for it."""
     if not randn.is_cuda:
         raise RuntimeError("sample_t23d runs on CUDA only (no CPU fallback)")
+    if s_churn > 0:
+        raise ValueError("sample_t23d does not fuse stochastic churn (s_churn > 0); use the sgm sampler classes")
+    if sampler != "EulerEDMSampler":
+        if tables is not None:
+            raise ValueError("tables= holds Euler-EDM coefficients; it cannot be used with sampler=" + repr(sampler))
+        plan = edm_sampler_plan(sampler, num_steps, scale, eta, s_noise, order)
+        return _sample_t23d_plan(model, randn, c, uc, plan, use_graph, noise)
+    if noise is not None:
+        raise ValueError("EulerEDMSampler draws no noise; noise= is for the ancestral samplers")
     B = randn.shape[0]
     if tables is None:
         tables = edm_cfg_tables(num_steps, scale, B, randn.device)
@@ -137,10 +317,11 @@ def decode_and_render(decoder, latents: torch.Tensor, cameras: torch.Tensor, res
 
 @torch.no_grad()
 def generate_t23d(model, decoder, randn, c, uc, cameras, num_steps: int = 250, scale: float = 6.5,
-                  resolution: int = 128):
+                  resolution: int = 128, sampler: str = "EulerEDMSampler", **sampler_kwargs):
     """Text-to-3D end to end on one GPU: sample -> decode -> render (the body of
-    DiffusionEngineLSGM.eval_cldm, nsr/lsgm/sgm_DiffusionEngine.py:410-523, minus conditioner + video sink)."""
-    latents = sample_t23d(model, randn, c, uc, num_steps, scale)
+    DiffusionEngineLSGM.eval_cldm, nsr/lsgm/sgm_DiffusionEngine.py:410-523, minus conditioner + video sink).
+    `sampler` and `sampler_kwargs` (eta, s_noise, order, noise) go to sample_t23d."""
+    latents = sample_t23d(model, randn, c, uc, num_steps, scale, sampler=sampler, **sampler_kwargs)
     return latents, decode_and_render(decoder, latents, cameras, resolution)
 
 
@@ -164,15 +345,17 @@ def condition_prompt(conditioner, cond_key: str, prompt, num_samples: int, devic
 
 @torch.no_grad()
 def text_to_3d(conditioner, model, decoder, prompt, cameras, num_samples: int = 1, num_steps: int = 250,
-               scale: float = 6.5, resolution: int = 128, seed: int = 41):
+               scale: float = 6.5, resolution: int = 128, seed: int = 41, sampler: str = "EulerEDMSampler",
+               **sampler_kwargs):
     """eval_cldm for one caption end to end (:410-523): conditioner -> `th.manual_seed(41)` CPU noise draw (:457-466,
-    395-398) -> Euler-EDM + CFG sampling -> decode -> render.  Returns (latents, render dict)."""
+    395-398) -> Euler-EDM + CFG sampling (or `sampler`, see sample_t23d) -> decode -> render.
+    Returns (latents, render dict)."""
     dev = next(model.parameters()).device
     c, uc = condition_prompt(conditioner, "caption", prompt, num_samples, device=dev)
     g = torch.Generator().manual_seed(seed)
     C = model.in_channels if not model.roll_out else 3 * model.in_channels
     randn = torch.randn(num_samples, C, 32, 32, generator=g).to(dev)
-    return generate_t23d(model, decoder, randn, c, uc, cameras, num_steps, scale, resolution)
+    return generate_t23d(model, decoder, randn, c, uc, cameras, num_steps, scale, resolution, sampler, **sampler_kwargs)
 
 
 @torch.no_grad()
