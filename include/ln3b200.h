@@ -388,8 +388,8 @@ int ln3_ode_step(const ln3_ode_args* args, void* stream);
 
 /* ------------------------------------------------------------------ tri-plane volumetric renderer
  * ln3_render_views: the whole of ImportanceRenderer.forward (nsr/volumetric_rendering/renderer.py:
- * 133-307) for the Objaverse preset (nsr/script_util.py:761-797): 'auto' ray limits against the
- * box (math_utils.py:124-190, renderer.py:145-155), 64 stratified + 64 importance samples per ray,
+ * 133-307) for the Objaverse presets (nsr/script_util.py:761-797, 838-870): 'auto' ray limits against the
+ * box (math_utils.py:124-190, renderer.py:145-155), S stratified + S importance samples per ray,
  * tri-plane bilinear gather (renderer.py:55-104), in-box filter (:381-405), OSGDecoder
  * (nsr/triplane.py:339-375, FullyConnectedLayer gains nsr/networks_stylegan2.py:141-145),
  * MipRayMarcher2 (ray_marcher.py:26-68), sample_importance / sample_pdf (:479-552) and
@@ -398,7 +398,9 @@ int ln3_ode_step(const ln3_ode_args* args, void* stream);
  *   planes_cl    fp32 [n_obj, 3, H, W, 32] channels-last (ln3_planes_to_channels_last)
  *   view_obj     int32 [V] object of each view, or NULL -> view v uses object v / views_per_obj
  *   ray_o, ray_d fp32 [V, M, 3]           (ln3_generate_rays, or caller supplied)
- *   noise_*      fp32 [V, M, 64] uniform [0,1): the tensors the reference draws with
+ *   S, S_importance  equal, 64 (objaverse_tuneray_aug_resolution_64_64_auto) or 96 (..._96_96_auto, the
+ *                preset of the DiT2-L/2 VAE); any other count is LN3_EUNSUPPORTED
+ *   noise_*      fp32 [V, M, S] uniform [0,1): the tensors the reference draws with
  *                torch.rand_like (renderer.py:464) and torch.rand (renderer.py:530)
  *   w1,b1,w2,b2  raw OSGDecoder parameters (64,32), (64), (4,64), (4) -- gains applied inside
  *   rgb          fp32 [V, 3, M]  ('feature_samples' permuted: image_raw when reshaped to H x W)
@@ -407,8 +409,8 @@ int ln3_ode_step(const ln3_ode_args* args, void* stream);
  * valid ray starts, depth clamp range): 1 when the reference renders one view per call
  * (nsr/train_util_diffusion.py:292-302), N for a batched Triplane.forward.
  * workspace: ln3_render_workspace_bytes(V, M, group_size) bytes of device memory.
- * dbg_* (optional, tests only): per-sample in-box masks [V*M,128] (coarse ++ fine), searchsorted
- * indices [V*M,64], sort permutation [V*M,128], fine depths [V*M,64].
+ * dbg_* (optional, tests only): per-sample in-box masks [V*M,2S] (coarse ++ fine), searchsorted
+ * indices [V*M,S], sort permutation [V*M,2S], fine depths [V*M,S].
  */
 typedef struct ln3_render_args {
   const float* planes_cl;
@@ -625,6 +627,15 @@ typedef struct ln3_vae_posterior_args {
 } ln3_vae_posterior_args;
 
 int ln3_vae_posterior(const ln3_vae_posterior_args* args, void* stream);
+
+/* ln3_view_mean_nhwc: the view pooling of MVEncoderGSDynamicInp (ldm/modules/diffusionmodules/model.py:611-623),
+ * feat.mean(keepdim=True, dim=0) over each object's F consecutive views:
+ *   x fp32 [B*F, S, S, C] NHWC -> out fp32 [B, S, S, C],
+ *   out[b, i] = (((x[b*F, i] + x[b*F + 1, i]) + ...) + x[b*F + F-1, i]) / F
+ * summed over the views in order in fp32, each addition rounded to nearest, then one IEEE division by F.
+ * LN3_EINVAL for F <= 0, B < 0, S <= 0, C <= 0 or a NULL x / out (checked before B == 0 returns without a
+ * launch).  out must not overlap x. */
+int ln3_view_mean_nhwc(const float* x, float* out, int B, int F, int S, int C, void* stream);
 
 /* ------------------------------------------------------------------ FP8 (e4m3) denoiser GEMMs
  * An opt-in operating point for the qkv / fc1 / fc2 GEMMs of the DiT blocks.  Its results are NOT held to the

@@ -331,6 +331,9 @@ int ln3_vae_posterior(const ln3_vae_posterior_args* args, void* stream) {
   if (!args) return set_error(LN3_EINVAL, "vae_posterior: null args");
   return vae_posterior(args, static_cast<cudaStream_t>(stream));
 }
+int ln3_view_mean_nhwc(const float* x, float* out, int B, int F, int S, int C, void* stream) {
+  return view_mean_nhwc(x, out, B, F, S, C, static_cast<cudaStream_t>(stream));
+}
 
 size_t ln3_ode_workspace_bytes(int B, long long n_per_sample) {
   if (B <= 0 || n_per_sample <= 0) return 0;

@@ -342,6 +342,34 @@ int vae_posterior(const ln3_vae_posterior_args* a, cudaStream_t stream) {
   return LN3_OK;
 }
 
+// ------------------------------------------------------------------ view mean (MVEncoderGSDynamicInp pooling)
+// feat.mean(keepdim=True, dim=0) over the F consecutive views of each object: one thread per output element,
+// consecutive threads on consecutive channels (coalesced reads of every view).  The sum runs over the views in
+// order in fp32 and is divided by F once (IEEE division).
+__global__ void __launch_bounds__(256)
+view_mean_kernel(const float* __restrict__ x, float* __restrict__ out, long long n_out, long long per_view, int F) {
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= n_out) return;
+  const long long b = i / per_view, r = i - b * per_view;
+  const float* src = x + b * F * per_view + r;
+  float s = __ldg(src);
+  for (int f = 1; f < F; ++f) s = __fadd_rn(s, __ldg(src + f * per_view));
+  out[i] = __fdiv_rn(s, static_cast<float>(F));
+}
+
+int view_mean_nhwc(const float* x, float* out, int B, int F, int S, int C, cudaStream_t stream) {
+  if (F <= 0 || B < 0 || S <= 0 || C <= 0) return set_error(LN3_EINVAL, "view_mean_nhwc: need F > 0, B >= 0, S > 0, C > 0");
+  if (!x || !out) return set_error(LN3_EINVAL, "view_mean_nhwc: null pointer");
+  if (B == 0) return LN3_OK;
+  const long long per_view = static_cast<long long>(S) * S * C, n = per_view * B;
+  if ((n + 255) / 256 > 0x7fffffffLL) return set_error(LN3_EINVAL, "view_mean_nhwc: B*S*S*C too large");
+  view_mean_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, stream>>>(x, out, n, per_view, F);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return set_error(LN3_ECUDA, "view_mean_nhwc launch: %s", cudaGetErrorString(e));
+  count_launch();
+  return LN3_OK;
+}
+
 // ------------------------------------------------------------------ GroupNorm statistics
 // One block per (image, group): mean / biased variance over H*W*(C/G) elements (two-pass, fp32 with
 // a shifted second pass for accuracy) -> per-channel scale = gamma*rstd, shift = beta - mean*scale.

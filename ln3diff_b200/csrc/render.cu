@@ -11,7 +11,9 @@
 //            (L1/L2 resident), blended feature rows staged in shared memory
 //   phase C (lane = sample): 32->64 softplus ->4 MLP from smem-resident weights, sigmoid / sigma
 //   then transmittance scan, importance resampling (cdf scan + binary search), second
-//   evaluation, rank-sort merge of the 64+64 samples and the final compositing scan.
+//   evaluation, rank-sort merge of the S+S samples and the final compositing scan.
+// S = S_importance is 64 (objaverse_tuneray_aug_resolution_64_64_auto) or 96 (..._96_96_auto, the DiT2-L/2
+// VAE's preset): a lane holds one sample of each of the S/32 blocks.
 // Global reductions of the reference (min/max of valid ray starts, renderer.py:151-155; depth clamp
 // range, ray_marcher.py:59-61) are per "group" of consecutive views (= one reference call) and
 // handled by a tiny pre-pass and finalize kernel.  Noise is an explicit input (the reference
@@ -24,7 +26,6 @@
 
 namespace ln3 {
 
-static constexpr int kS = 64;          // coarse == importance sample count (objaverse preset)
 static constexpr int kC = 32;          // plane feature channels
 static constexpr int kHid = 64;        // OSG hidden width
 static constexpr int kWarpsPerBlock = 16;  // one 512-thread CTA per SM: a 4x4 pixel tile of rays marches in lock-step
@@ -118,27 +119,34 @@ struct RenderParams {
   int white_back;
   int mlp_tf32;   // 1: OSG MLP on the tensor cores (TF32 operands, fp32 accumulate); 0: exact fp32 SIMT
   int no_filter;  // 1: raw decoder output for every point (ImportanceRenderer._run_model), no in-box filter
-  // optional debug outputs (tests): in-box masks / importance indices / sort permutation
-  unsigned char* dbg_inbox;  // [V*M][128]
-  int* dbg_inds;             // [V*M][64]
-  int* dbg_order;            // [V*M][128]
-  float* dbg_zfine;          // [V*M][64]
+  // optional debug outputs (tests): in-box masks / importance indices / sort permutation, S samples per pass
+  unsigned char* dbg_inbox;  // [V*M][2S]
+  int* dbg_inds;             // [V*M][S]
+  int* dbg_order;            // [V*M][2S]
+  float* dbg_zfine;          // [V*M][S]
 };
 
-struct WarpSmem {
+// Per-warp buffers of one 32-sample model evaluation (eval_batch).
+struct GatherSmem {
   int tap_off[32][12];
   float tap_w[32][12];
   float feat[32][36];   // stride 36: A-fragment reads (row g, col t) hit 32 distinct banks; rows 16-B aligned
-  float cdf[64];
-  float bins[64];
-  float sz[128];   // merged samples: depth, sigma, r, g, b
-  float ss[128];
-  float sr[128];
-  float sg[128];
-  float sb[128];
 };
 
-struct BlockSmem {
+template <int S>
+struct WarpSmem {
+  GatherSmem g;
+  float cdf[S];
+  float bins[S];
+  float sz[2 * S];   // merged samples: depth, sigma, r, g, b
+  float ss[2 * S];
+  float sr[2 * S];
+  float sg[2 * S];
+  float sb[2 * S];
+};
+static_assert(2 * 96 <= 32 * 36, "the unify stage stages 2S depths in GatherSmem::feat");
+
+struct OsgSmem {
   float w1[kHid][kC];  // pre-scaled by 1/sqrt(32)
   float b1[kHid];
   float w2[4][kHid];   // pre-scaled by 1/8
@@ -146,11 +154,18 @@ struct BlockSmem {
   // TF32 tensor-core path: the same weights as mma.m16n8k8 B fragments (tf32-rounded), one float2 per lane
   float2 w1f[8][4][32];  // [n-tile of 8 hidden units][k-step of 8 features][lane] = (b0, b1)
   float2 w2f[8][32];     // [k-step = layer-1 n-tile][lane]; hidden units in layer-1 accumulator order
-  WarpSmem warp[kWarpsPerBlock];
 };
 
+// 191,760 B at S = 64 and 216,336 B at S = 96: both fit the 232,448 B opt-in limit with 16 warps per CTA.
+template <int S>
+struct BlockSmem {
+  OsgSmem osg;
+  WarpSmem<S> warp[kWarpsPerBlock];
+};
+static_assert(sizeof(BlockSmem<96>) <= 232448, "S = 96 must fit one 16-warp CTA per SM");
+
 // Fill the weight copies of a block (fp32 rows for the SIMT path, tf32 B fragments for the mma path).
-__device__ __forceinline__ void load_osg_weights(BlockSmem& bs, const float* w1, const float* b1, const float* w2,
+__device__ __forceinline__ void load_osg_weights(OsgSmem& bs, const float* w1, const float* b1, const float* w2,
                                                  const float* b2) {
   for (int i = threadIdx.x; i < kHid * kC; i += blockDim.x)
     (&bs.w1[0][0])[i] = __fmul_rn(w1[i], 0.17677669529663687f);  // weight_gain = 1/sqrt(32)
@@ -238,7 +253,7 @@ __device__ __forceinline__ void plane_taps(float gx, float gy, int H, int W, int
 // miss) became the top stall once the MLP moved to the tensor cores; the precision is a template
 // parameter so that only one MLP body is in the instruction stream.
 template <bool TF32>
-__device__ __noinline__ void eval_batch(const RenderParams& p, const BlockSmem& bs, WarpSmem& ws,
+__device__ __noinline__ void eval_batch(const RenderParams& p, const OsgSmem& bs, GatherSmem& ws,
                                            const float* __restrict__ planes_obj, int lane,
                                            float px, float py, float pz, bool& inbox, float& sigma,
                                            float& cr, float& cg, float& cb) {
@@ -404,15 +419,16 @@ __device__ __noinline__ void eval_batch(const RenderParams& p, const BlockSmem& 
 // 64 KB of L1 left beside the shared-memory carve-out only helps rays that are co-resident in space AND time.
 // There is no barrier per item: rays that miss the volume skip the gather and the MLP (eval_batch) and their
 // warps simply move on to the next tile.
-template <bool TF32>
+template <bool TF32, int NB>
 __global__ void __launch_bounds__(kWarpsPerBlock * 32, 1)
 render_rays_kernel(const RenderParams p) {
+  constexpr int S = 32 * NB;  // coarse == importance sample count
   extern __shared__ uint8_t smem_raw[];
-  BlockSmem& bs = *reinterpret_cast<BlockSmem*>(smem_raw);
+  BlockSmem<S>& bs = *reinterpret_cast<BlockSmem<S>*>(smem_raw);
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  load_osg_weights(bs, p.w1, p.b1, p.w2, p.b2);
+  load_osg_weights(bs.osg, p.w1, p.b1, p.w2, p.b2);
   __syncthreads();
-  WarpSmem& ws = bs.warp[warp];
+  WarpSmem<S>& ws = bs.warp[warp];
 
   const long long total = static_cast<long long>(p.V) * p.M;
   const int tiles_x = p.image_w > 0 ? p.image_w / 4 : 0;
@@ -445,141 +461,168 @@ render_rays_kernel(const RenderParams p) {
     }
     // ---- stratified coarse depths (renderer.py:455-466, math_utils.linspace)
     const float span = __fsub_rn(end, start);
-    const float delta = __fdiv_rn(span, static_cast<float>(kS - 1));
-    float zc[2];
+    const float delta = __fdiv_rn(span, static_cast<float>(S - 1));
+    float zc[NB];
 #pragma unroll
-    for (int b = 0; b < 2; ++b) {
+    for (int b = 0; b < NB; ++b) {
       const int j = b * 32 + lane;
-      const float step = __fdiv_rn(static_cast<float>(j), static_cast<float>(kS - 1));
+      const float step = __fdiv_rn(static_cast<float>(j), static_cast<float>(S - 1));
       const float base = __fadd_rn(start, __fmul_rn(step, span));
-      zc[b] = __fadd_rn(base, __fmul_rn(p.noise_c[ray * kS + j], delta));
+      zc[b] = __fadd_rn(base, __fmul_rn(p.noise_c[ray * S + j], delta));
     }
-    float sc[2], rc[2], gc[2], bc[2];
+    float sc[NB], rc[NB], gc[NB], bc[NB];
 #pragma unroll
-    for (int b = 0; b < 2; ++b) {
+    for (int b = 0; b < NB; ++b) {
       const float px = __fadd_rn(ox, __fmul_rn(zc[b], dx));
       const float py = __fadd_rn(oy, __fmul_rn(zc[b], dy));
       const float pz = __fadd_rn(oz, __fmul_rn(zc[b], dz));
       bool inbox;
-      eval_batch<TF32>(p, bs, ws, planes_obj, lane, px, py, pz, inbox, sc[b], rc[b], gc[b], bc[b]);
-      if (p.dbg_inbox) p.dbg_inbox[ray * 128 + b * 32 + lane] = inbox;
+      eval_batch<TF32>(p, bs.osg, ws.g, planes_obj, lane, px, py, pz, inbox, sc[b], rc[b], gc[b], bc[b]);
+      if (p.dbg_inbox) p.dbg_inbox[ray * (2 * S) + b * 32 + lane] = inbox;
     }
     // ---- coarse ray march -> weights (ray_marcher.py:26-47); interval i = samples (i, i+1)
-    float wgt[2];  // weight of interval b*32+lane (interval 63 does not exist)
+    float wgt[NB];  // weight of interval b*32+lane (interval S-1 does not exist)
     {
-      float alpha[2], om[2];
+      float alpha[NB], om[NB];
 #pragma unroll
-      for (int b = 0; b < 2; ++b) {
+      for (int b = 0; b < NB; ++b) {
         float zn = __shfl_down_sync(0xffffffffu, zc[b], 1);
         float sn = __shfl_down_sync(0xffffffffu, sc[b], 1);
-        if (b == 0) {
-          const float z32 = __shfl_sync(0xffffffffu, zc[1], 0), s32 = __shfl_sync(0xffffffffu, sc[1], 0);
+        if (b < NB - 1) {
+          const float z32 = __shfl_sync(0xffffffffu, zc[b + 1], 0), s32 = __shfl_sync(0xffffffffu, sc[b + 1], 0);
           if (lane == 31) { zn = z32; sn = s32; }
         }
-        const bool has = (b == 0) || (lane < 31);
+        const bool has = (b < NB - 1) || (lane < 31);
         const float dlt = zn - zc[b];
         const float smid = softplus_t((sc[b] + sn) / 2.f - 1.f);
         alpha[b] = has ? 1.f - expf(-(smid * dlt)) : 0.f;
         om[b] = has ? (1.f - alpha[b]) + 1e-10f : 1.f;
       }
-      const float inc0 = warp_incl_prod(om[0], lane);
-      const float tot0 = __shfl_sync(0xffffffffu, inc0, 31);
-      const float inc1 = warp_incl_prod(om[1], lane) * tot0;
-      float ex0 = __shfl_up_sync(0xffffffffu, inc0, 1);
-      float ex1 = __shfl_up_sync(0xffffffffu, inc1, 1);
-      if (lane == 0) { ex0 = 1.f; ex1 = tot0; }
-      wgt[0] = alpha[0] * ex0;
-      wgt[1] = alpha[1] * ex1;
+      // transmittance: inclusive product per block, chained across blocks by the previous blocks' total
+      float inc[NB], tot[NB];
+#pragma unroll
+      for (int b = 0; b < NB; ++b) {
+        inc[b] = warp_incl_prod(om[b], lane);
+        if (b > 0) inc[b] *= tot[b - 1];
+        if (b < NB - 1) tot[b] = __shfl_sync(0xffffffffu, inc[b], 31);
+      }
+#pragma unroll
+      for (int b = 0; b < NB; ++b) {
+        float ex = __shfl_up_sync(0xffffffffu, inc[b], 1);
+        if (lane == 0) ex = b > 0 ? tot[b - 1] : 1.f;
+        wgt[b] = alpha[b] * ex;
+      }
     }
     // ---- importance sampling (renderer.py:479-552)
-    float zf[2];
+    float zf[NB];
     {
-      // smoothed[i] = (max(w[i-1], w[i]) + max(w[i], w[i+1])) / 2 + 0.01 for i = 0..62 (w[-1] = w[63] = -inf)
-      float sm[2];
+      // smoothed[i] = (max(w[i-1], w[i]) + max(w[i], w[i+1])) / 2 + 0.01 for i = 0..S-2 (w[-1] = w[S-1] = -inf)
+      float sm[NB];
 #pragma unroll
-      for (int b = 0; b < 2; ++b) {
+      for (int b = 0; b < NB; ++b) {
         float prev = __shfl_up_sync(0xffffffffu, wgt[b], 1);
         float next = __shfl_down_sync(0xffffffffu, wgt[b], 1);
-        if (b == 0) {
-          const float w32 = __shfl_sync(0xffffffffu, wgt[1], 0);
+        if (b < NB - 1) {
+          const float w32 = __shfl_sync(0xffffffffu, wgt[b + 1], 0);
           if (lane == 31) next = w32;
+        }
+        if (b == 0) {
           if (lane == 0) prev = -INFINITY;
         } else {
-          const float w31 = __shfl_sync(0xffffffffu, wgt[0], 31);
+          const float w31 = __shfl_sync(0xffffffffu, wgt[b - 1], 31);
           if (lane == 0) prev = w31;
-          if (lane >= 30) next = -INFINITY;  // interval 62's right neighbour is the pad
         }
+        if (b == NB - 1 && lane >= 30) next = -INFINITY;  // interval S-2's right neighbour is the pad
         sm[b] = (fmaxf(prev, wgt[b]) + fmaxf(wgt[b], next)) / 2.f + 0.01f;
       }
-      // pdf over smoothed[1..61] (61 weights), bins = mid-points of the 64 coarse depths (63)
-      float wv[2];
-      wv[0] = (lane >= 1) ? sm[0] + 1e-5f : 0.f;   // index lane     in 1..31
-      wv[1] = (lane <= 29) ? sm[1] + 1e-5f : 0.f;  // index 32+lane  in 32..61
-      const float tot = warp_sum_f(wv[0]) + warp_sum_f(wv[1]);
-      const float pdf0 = wv[0] / tot, pdf1 = wv[1] / tot;
-      const float c0 = warp_incl_sum(pdf0, lane);
-      const float c0tot = __shfl_sync(0xffffffffu, c0, 31);
-      const float c1 = warp_incl_sum(pdf1, lane) + c0tot;
-      // cdf[0] = 0, cdf[k] = sum of pdf over smoothed[1..k], k = 1..61  (62 entries)
-      ws.cdf[lane] = (lane == 0) ? 0.f : c0;
-      if (lane <= 29) ws.cdf[32 + lane] = c1;
-      // bins (z_mid) 0..62
+      // pdf over smoothed[1..S-3] (S-3 weights), bins = mid-points of the S coarse depths (S-1)
+      float wv[NB];
 #pragma unroll
-      for (int b = 0; b < 2; ++b) {
+      for (int b = 0; b < NB; ++b) {  // index b*32+lane in 1..S-3
+        const bool in = (b > 0 || lane >= 1) && (b < NB - 1 || lane <= 29);
+        wv[b] = in ? sm[b] + 1e-5f : 0.f;
+      }
+      float tot = warp_sum_f(wv[0]);
+#pragma unroll
+      for (int b = 1; b < NB; ++b) tot += warp_sum_f(wv[b]);
+      float pdf[NB];
+#pragma unroll
+      for (int b = 0; b < NB; ++b) pdf[b] = wv[b] / tot;
+      float c[NB];
+#pragma unroll
+      for (int b = 0; b < NB; ++b) {
+        c[b] = warp_incl_sum(pdf[b], lane);
+        if (b > 0) c[b] += __shfl_sync(0xffffffffu, c[b - 1], 31);
+      }
+      // cdf[0] = 0, cdf[k] = sum of pdf over smoothed[1..k], k = 1..S-3  (S-2 entries)
+      ws.cdf[lane] = (lane == 0) ? 0.f : c[0];
+#pragma unroll
+      for (int b = 1; b < NB; ++b)
+        if (b < NB - 1 || lane <= 29) ws.cdf[b * 32 + lane] = c[b];
+      // bins (z_mid) 0..S-2
+#pragma unroll
+      for (int b = 0; b < NB; ++b) {
         float zn = __shfl_down_sync(0xffffffffu, zc[b], 1);
-        if (b == 0) {
-          const float z32 = __shfl_sync(0xffffffffu, zc[1], 0);
+        if (b < NB - 1) {
+          const float z32 = __shfl_sync(0xffffffffu, zc[b + 1], 0);
           if (lane == 31) zn = z32;
         }
-        if (b == 0 || lane < 31) ws.bins[b * 32 + lane] = 0.5f * (zc[b] + zn);
+        if (b < NB - 1 || lane < 31) ws.bins[b * 32 + lane] = 0.5f * (zc[b] + zn);
       }
       __syncwarp();
 #pragma unroll
-      for (int b = 0; b < 2; ++b) {
-        const float u = p.noise_f[ray * kS + b * 32 + lane];
-        // searchsorted(cdf[0..61], u, right=True): first index with cdf > u
-        int lo = 0, hi = 62;
+      for (int b = 0; b < NB; ++b) {
+        const float u = p.noise_f[ray * S + b * 32 + lane];
+        // searchsorted(cdf[0..S-3], u, right=True): first index with cdf > u
+        int lo = 0, hi = S - 2;
         while (lo < hi) {
           const int mid = (lo + hi) >> 1;
           if (ws.cdf[mid] <= u) lo = mid + 1; else hi = mid;
         }
-        const int below = max(lo - 1, 0), above = min(lo, 61);
+        const int below = max(lo - 1, 0), above = min(lo, S - 3);
         const float cb0 = ws.cdf[below], cb1 = ws.cdf[above];
         const float bb0 = ws.bins[below], bb1 = ws.bins[above];
         float den = cb1 - cb0;
         if (den < 1e-5f) den = 1.f;
         zf[b] = bb0 + (u - cb0) / den * (bb1 - bb0);
-        if (p.dbg_inds) p.dbg_inds[ray * kS + b * 32 + lane] = lo;
-        if (p.dbg_zfine) p.dbg_zfine[ray * kS + b * 32 + lane] = zf[b];
+        if (p.dbg_inds) p.dbg_inds[ray * S + b * 32 + lane] = lo;
+        if (p.dbg_zfine) p.dbg_zfine[ray * S + b * 32 + lane] = zf[b];
       }
       __syncwarp();
     }
     // ---- fine pass
-    float sf[2], rf[2], gf[2], bf[2];
+    float sf[NB], rf[NB], gf[NB], bf[NB];
 #pragma unroll
-    for (int b = 0; b < 2; ++b) {
+    for (int b = 0; b < NB; ++b) {
       const float px = __fadd_rn(ox, __fmul_rn(zf[b], dx));
       const float py = __fadd_rn(oy, __fmul_rn(zf[b], dy));
       const float pz = __fadd_rn(oz, __fmul_rn(zf[b], dz));
       bool inbox;
-      eval_batch<TF32>(p, bs, ws, planes_obj, lane, px, py, pz, inbox, sf[b], rf[b], gf[b], bf[b]);
-      if (p.dbg_inbox) p.dbg_inbox[ray * 128 + 64 + b * 32 + lane] = inbox;
+      eval_batch<TF32>(p, bs.osg, ws.g, planes_obj, lane, px, py, pz, inbox, sf[b], rf[b], gf[b], bf[b]);
+      if (p.dbg_inbox) p.dbg_inbox[ray * (2 * S) + S + b * 32 + lane] = inbox;
     }
-    // ---- unify: stable rank sort of the 128 (coarse ++ fine) depths (renderer.py:422-435)
+    // ---- unify: stable rank sort of the 2S (coarse ++ fine) depths (renderer.py:422-435)
+    constexpr int Q = 2 * NB;  // 32-sample blocks of the merged ray
     {
-      float* stage = &ws.feat[0][0];  // 128 unsorted depths
-      stage[lane] = zc[0];
-      stage[32 + lane] = zc[1];
-      stage[64 + lane] = zf[0];
-      stage[96 + lane] = zf[1];
+      float* stage = &ws.g.feat[0][0];  // 2S unsorted depths
+#pragma unroll
+      for (int b = 0; b < NB; ++b) {
+        stage[b * 32 + lane] = zc[b];
+        stage[S + b * 32 + lane] = zf[b];
+      }
       __syncwarp();
-      int rank[4] = {0, 0, 0, 0};
-      const float mine[4] = {zc[0], zc[1], zf[0], zf[1]};
+      int rank[Q];
+      float mine[Q];
+#pragma unroll
+      for (int q = 0; q < Q; ++q) {
+        rank[q] = 0;
+        mine[q] = q < NB ? zc[q % NB] : zf[q % NB];
+      }
       // rank = #(z_k < mine) + #(z_k == mine with k < my index).  My index is q*32 + lane, so against a
       // whole 32-block kb the tie-break is a compile-time choice (kb < q: "<=", kb > q: "<") and only the
       // own block needs the lane-dependent form; candidates come four per LDS.128.
 #pragma unroll
-      for (int kb = 0; kb < 4; ++kb) {
+      for (int kb = 0; kb < Q; ++kb) {
 #pragma unroll 2
         for (int kk = 0; kk < 32; kk += 4) {
           const float4 z4 = *reinterpret_cast<const float4*>(stage + kb * 32 + kk);
@@ -588,7 +631,7 @@ render_rays_kernel(const RenderParams p) {
           for (int e = 0; e < 4; ++e) {
             const float zk = zs[e];
 #pragma unroll
-            for (int q = 0; q < 4; ++q) {
+            for (int q = 0; q < Q; ++q) {
               if (kb < q) rank[q] += zk <= mine[q];
               else if (kb > q) rank[q] += zk < mine[q];
               else rank[q] += (zk < mine[q]) || (zk == mine[q] && kk + e < lane);
@@ -596,29 +639,26 @@ render_rays_kernel(const RenderParams p) {
           }
         }
       }
-      const float sv[4] = {sc[0], sc[1], sf[0], sf[1]};
-      const float rv[4] = {rc[0], rc[1], rf[0], rf[1]};
-      const float gv[4] = {gc[0], gc[1], gf[0], gf[1]};
-      const float bv[4] = {bc[0], bc[1], bf[0], bf[1]};
 #pragma unroll
-      for (int q = 0; q < 4; ++q) {
+      for (int q = 0; q < Q; ++q) {
+        const int b = q % NB;
         ws.sz[rank[q]] = mine[q];
-        ws.ss[rank[q]] = sv[q];
-        ws.sr[rank[q]] = rv[q];
-        ws.sg[rank[q]] = gv[q];
-        ws.sb[rank[q]] = bv[q];
-        if (p.dbg_order) p.dbg_order[ray * 128 + rank[q]] = q * 32 + lane;
+        ws.ss[rank[q]] = q < NB ? sc[b] : sf[b];
+        ws.sr[rank[q]] = q < NB ? rc[b] : rf[b];
+        ws.sg[rank[q]] = q < NB ? gc[b] : gf[b];
+        ws.sb[rank[q]] = q < NB ? bc[b] : bf[b];
+        if (p.dbg_order) p.dbg_order[ray * (2 * S) + rank[q]] = q * 32 + lane;
       }
       __syncwarp();
     }
-    // ---- final march over 127 intervals (ray_marcher.py:26-68)
+    // ---- final march over 2S-1 intervals (ray_marcher.py:26-68)
     float acc_r = 0.f, acc_g = 0.f, acc_b = 0.f, acc_d = 0.f, acc_w = 0.f;
     {
       float carry = 1.f;
 #pragma unroll
-      for (int q = 0; q < 4; ++q) {
+      for (int q = 0; q < Q; ++q) {
         const int i = q * 32 + lane;
-        const bool has = i < 127;
+        const bool has = i < 2 * S - 1;
         const int i1 = has ? i + 1 : i;
         const float z0 = ws.sz[i], z1 = ws.sz[i1];
         const float smid = softplus_t((ws.ss[i] + ws.ss[i1]) / 2.f - 1.f);
@@ -656,7 +696,7 @@ render_rays_kernel(const RenderParams p) {
       p.depth[ray] = acc_d;  // clamped by render_finalize_kernel
       p.wsum[ray] = acc_w;
       atomicMin(&p.keys[grp * 4 + 2], float_key(ws.sz[0]));
-      atomicMax(&p.keys[grp * 4 + 3], float_key(ws.sz[127]));
+      atomicMax(&p.keys[grp * 4 + 3], float_key(ws.sz[2 * S - 1]));
     }
     __syncwarp();
   }
@@ -684,10 +724,31 @@ size_t render_workspace_bytes(int V, int M, int group_size) {
   return static_cast<size_t>(G) * 4 * sizeof(int) + static_cast<size_t>(V) * M * 2 * sizeof(float) + 256;
 }
 
+// One instantiation per (MLP precision, samples per ray): the dynamic shared memory is opted in per kernel.
+template <int NB>
+static int launch_render_rays(const RenderParams& p, long long blocks, cudaStream_t stream) {
+  constexpr size_t smem = sizeof(BlockSmem<32 * NB>);
+  static DeviceOnce once;
+  if (int rc = once.run([] {
+        cudaError_t e = cudaFuncSetAttribute(render_rays_kernel<false, NB>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                             static_cast<int>(smem));
+        if (e == cudaSuccess)
+          e = cudaFuncSetAttribute(render_rays_kernel<true, NB>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   static_cast<int>(smem));
+        return e == cudaSuccess ? LN3_OK : set_error(LN3_ECUDA, "render: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
+      }))
+    return rc;
+  if (p.mlp_tf32)
+    render_rays_kernel<true, NB><<<static_cast<unsigned>(blocks), kWarpsPerBlock * 32, smem, stream>>>(p);
+  else
+    render_rays_kernel<false, NB><<<static_cast<unsigned>(blocks), kWarpsPerBlock * 32, smem, stream>>>(p);
+  return LN3_OK;
+}
+
 int render_views(const ln3_render_args* a, cudaStream_t stream) {
   if (a->V <= 0 || a->M <= 0) return LN3_OK;
-  if (a->C != kC || a->S != kS || a->S_importance != kS)
-    return set_error(LN3_EUNSUPPORTED, "render: needs 32 plane channels and 64+64 samples per ray");
+  if (a->C != kC || a->S != a->S_importance || (a->S != 64 && a->S != 96))
+    return set_error(LN3_EUNSUPPORTED, "render: needs 32 plane channels and 64+64 or 96+96 samples per ray");
   if (a->decoder_output_dim != 3 || a->hidden_dim != kHid)
     return set_error(LN3_EUNSUPPORTED, "render: OSG decoder must be 32 -> 64 -> 1+3");
   if (a->group_size <= 0) return set_error(LN3_EINVAL, "render: group_size must be > 0");
@@ -731,23 +792,11 @@ int render_views(const ln3_render_args* a, cudaStream_t stream) {
   p.dbg_inbox = a->dbg_inbox; p.dbg_inds = a->dbg_inds; p.dbg_order = a->dbg_order;
   p.dbg_zfine = a->dbg_zfine;
 
-  static DeviceOnce once;
-  if (int rc = once.run([] {
-        cudaError_t e = cudaFuncSetAttribute(render_rays_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                             static_cast<int>(sizeof(BlockSmem)));
-        if (e == cudaSuccess)
-          e = cudaFuncSetAttribute(render_rays_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                   static_cast<int>(sizeof(BlockSmem)));
-        return e == cudaSuccess ? LN3_OK : set_error(LN3_ECUDA, "render: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
-      }))
-    return rc;
   const int sms = device_sm_count();
   long long blocks = (rays + kWarpsPerBlock - 1) / kWarpsPerBlock;
   if (blocks > sms) blocks = sms;  // persistent: one 16-warp CTA per SM, grid-stride over 16-ray items
-  if (p.mlp_tf32)
-    render_rays_kernel<true><<<static_cast<unsigned>(blocks), kWarpsPerBlock * 32, sizeof(BlockSmem), stream>>>(p);
-  else
-    render_rays_kernel<false><<<static_cast<unsigned>(blocks), kWarpsPerBlock * 32, sizeof(BlockSmem), stream>>>(p);
+  if (int rc = a->S == 64 ? launch_render_rays<2>(p, blocks, stream) : launch_render_rays<3>(p, blocks, stream))
+    return rc;
   render_finalize_kernel<<<static_cast<unsigned>((rays + 255) / 256), 256, 0, stream>>>(
       a->depth, keys, a->V, a->M, a->group_size);
   cudaError_t e = cudaGetLastError();
@@ -780,11 +829,11 @@ template <bool TF32>
 __global__ void __launch_bounds__(kWarpsPerBlock * 32, 1)
 query_points_kernel(const RenderParams p, const QueryParams q) {
   extern __shared__ uint8_t smem_raw[];
-  BlockSmem& bs = *reinterpret_cast<BlockSmem*>(smem_raw);
+  BlockSmem<64>& bs = *reinterpret_cast<BlockSmem<64>*>(smem_raw);
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  load_osg_weights(bs, p.w1, p.b1, p.w2, p.b2);
+  load_osg_weights(bs.osg, p.w1, p.b1, p.w2, p.b2);
   __syncthreads();
-  WarpSmem& ws = bs.warp[warp];
+  WarpSmem<64>& ws = bs.warp[warp];
   const long long chunks_per_obj = (q.P + 31) / 32;
   const long long total = chunks_per_obj * q.n_obj;
   const long long stride = static_cast<long long>(gridDim.x) * kWarpsPerBlock;
@@ -807,7 +856,7 @@ query_points_kernel(const RenderParams p, const QueryParams q) {
     const float* planes_obj = p.planes + static_cast<long long>(obj) * 3 * p.H * p.W * kC;
     bool inbox;
     float sg, cr, cg, cb;
-    eval_batch<TF32>(p, bs, ws, planes_obj, lane, px, py, pz, inbox, sg, cr, cg, cb);
+    eval_batch<TF32>(p, bs.osg, ws.g, planes_obj, lane, px, py, pz, inbox, sg, cr, cg, cb);
     if (live) {
       const long long o = static_cast<long long>(obj) * q.P + i;
       q.sigma[o] = sg;
@@ -857,10 +906,10 @@ int query_points(const ln3_query_points_args* a, cudaStream_t stream) {
   static DeviceOnce once;
   if (int rc = once.run([] {
         cudaError_t e = cudaFuncSetAttribute(query_points_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                             static_cast<int>(sizeof(BlockSmem)));
+                                             static_cast<int>(sizeof(BlockSmem<64>)));
         if (e == cudaSuccess)
           e = cudaFuncSetAttribute(query_points_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                   static_cast<int>(sizeof(BlockSmem)));
+                                   static_cast<int>(sizeof(BlockSmem<64>)));
         return e == cudaSuccess ? LN3_OK : set_error(LN3_ECUDA, "query_points: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
       }))
     return rc;
@@ -869,9 +918,9 @@ int query_points(const ln3_query_points_args* a, cudaStream_t stream) {
   const int sms = device_sm_count();
   if (blocks > sms) blocks = sms;  // one 16-warp CTA per SM
   if (p.mlp_tf32)
-    query_points_kernel<true><<<static_cast<unsigned>(blocks), kWarpsPerBlock * 32, sizeof(BlockSmem), stream>>>(p, q);
+    query_points_kernel<true><<<static_cast<unsigned>(blocks), kWarpsPerBlock * 32, sizeof(BlockSmem<64>), stream>>>(p, q);
   else
-    query_points_kernel<false><<<static_cast<unsigned>(blocks), kWarpsPerBlock * 32, sizeof(BlockSmem), stream>>>(p, q);
+    query_points_kernel<false><<<static_cast<unsigned>(blocks), kWarpsPerBlock * 32, sizeof(BlockSmem<64>), stream>>>(p, q);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error(LN3_ECUDA, "query_points launch: %s", cudaGetErrorString(e));
   count_launch();

@@ -3,8 +3,9 @@ its blocks (ResnetBlock :94-153, Upsample :54-69, MemoryEfficientAttnBlock :209-
 containers with the reference's state_dict keys.  The arithmetic runs in
 ln3diff_b200.vit.vit_triplane on the NHWC fp32 conv kernels of libln3b200.
 
-The stage-1 VAE encoder `MVEncoder` (:459-577, Downsample :72-91, mid-block SpatialTransformer3D of
-ldm/modules/attention.py:390-463) is built here with its own NHWC forward: convolutions on ln3_conv_nhwc /
+The stage-1 VAE encoders `MVEncoder` (:459-577, Downsample :72-91, mid-block SpatialTransformer3D of
+ldm/modules/attention.py:390-463) and `MVEncoderGSDynamicInp` (:604-623, the DiT2-L/2 VAE's encoder) are built here
+with their own NHWC forward: one shared trunk, then a conv fusion or a mean over the views.  Convolutions on ln3_conv_nhwc /
 ln3_downsample_nhwc (TF32 by default, `conv_tf32 = False` for exact fp32), the multi-view transformer on the bf16
 wgmma GEMM and attention kernels with fp32 accumulation and an fp32 residual stream."""
 import torch
@@ -156,15 +157,15 @@ class SpatialTransformer3D(nn.Module):
         self.use_linear = False
 
 
-class MVEncoder(nn.Module):
-    """model.py:563-577: the SD `Encoder` (:459-560) with the 'mv-vanilla' mid-block attention, plus a conv fusion of
-    the 4 views of each object (pixel-nerf style).  Parameters as the reference's; forward on the NHWC kernels.  The
-    reference's single-view `Encoder` (ShapeNet / FFHQ configurations, outside the release inference paths) is not
-    mirrored and keeps resolving to the reference's own class under the overlay."""
+class _MVEncoderTrunk(nn.Module):
+    """The SD `Encoder` (model.py:459-560) with the 'mv-vanilla' mid-block attention, as the multi-view encoders build
+    it: parameters as the reference's, forward on the NHWC kernels.  The reference's single-view `Encoder` (ShapeNet /
+    FFHQ configurations, outside the release inference paths) is not mirrored and keeps resolving to the reference's
+    own class under the overlay."""
 
     def __init__(self, *, ch, out_ch, ch_mult=(1, 2, 4, 8), num_res_blocks, attn_resolutions, dropout=0,
                  resamp_with_conv=True, in_channels, resolution, z_channels, double_z=True, use_linear_attn=False,
-                 attn_type="mv-vanilla", attn_kwargs={}, **ignore_kwargs):
+                 attn_type="mv-vanilla", attn_kwargs={}, add_fusion_layer=False, **ignore_kwargs):
         super().__init__()
         if attn_type != "mv-vanilla" or attn_resolutions or use_linear_attn or dropout:
             raise NotImplementedError("attn_type other than 'mv-vanilla', attn_resolutions, linear attention and dropout "
@@ -196,8 +197,8 @@ class MVEncoder(nn.Module):
         self.norm_out = Normalize(block_in)
         zc = 2 * z_channels if double_z else z_channels
         self.conv_out = nn.Conv2d(block_in, zc, kernel_size=3, stride=1, padding=1)
-        self.fusion_layer = nn.Conv2d(zc * 4, zc, kernel_size=3, stride=1, padding=1)
-        self.num_frames = 4
+        if add_fusion_layer:
+            self.fusion_layer = nn.Conv2d(zc * 4, zc, kernel_size=3, stride=1, padding=1)
         self._prep = None
 
     # ------------------------------------------------------------------ weight repack
@@ -244,8 +245,9 @@ class MVEncoder(nn.Module):
                     ff_v=(bf(g.weight[:4 * inner]), f32(g.bias[:4 * inner])),
                     ff_g=(bf(g.weight[4 * inner:]), f32(g.bias[4 * inner:])),
                     ff_o=(bf(tb.ff.net[2].weight), f32(tb.ff.net[2].bias))),
-            norm_out=(f32(self.norm_out.weight), f32(self.norm_out.bias)), conv_out=pk(self.conv_out),
-            fusion=pk(self.fusion_layer))
+            norm_out=(f32(self.norm_out.weight), f32(self.norm_out.bias)), conv_out=pk(self.conv_out))
+        if hasattr(self, "fusion_layer"):
+            self._prep["fusion"] = pk(self.fusion_layer)
         return self._prep
 
     # ------------------------------------------------------------------ forward (NHWC)
@@ -294,15 +296,15 @@ class MVEncoder(nn.Module):
         ops.gemm(a, *P["ff_v"], out_kind=ops.OUT_RESID_F32, out=prod, gate=gate, gate_rows=1, out2=prod_bf)
         return prod, prod_bf
 
-    @torch.no_grad()
-    def forward_nhwc(self, x):
-        """x (B*F, in_channels, R, R) fp32 CUDA -> fused moments (B, R/8, R/8, 2*z_channels) NHWC fp32."""
+    def _trunk_nhwc(self, x, num_frames: int):
+        """Encoder.forward (model.py:526-560) with the mid-block attention over groups of `num_frames` views:
+        x (B*F, in_channels, R, R) fp32 CUDA -> per-view moments (B*F, R/8, R/8, 2*z_channels) NHWC fp32."""
         if not x.is_cuda:
             raise RuntimeError("ln3diff_b200 encoder runs on CUDA only (no CPU fallback)")
         if self._prep is None:
             self.prepare()
         P = self._prep
-        F_ = self.num_frames
+        F_ = num_frames
         assert x.dim() == 4 and x.shape[0] % F_ == 0 and x.shape[1] == self.in_channels, "x must be (B*views, C, H, W)"
         tf = self.conv_tf32
         h = x.float().permute(0, 2, 3, 1).contiguous()                         # NCHW -> NHWC (plumbing copy)
@@ -315,11 +317,31 @@ class MVEncoder(nn.Module):
         h = self._res(h, P["mid1"])
         h = self._spatial_transformer(h, P["st"], F_)
         h = self._res(h, P["mid2"])
-        h = ops.conv_nhwc(h, *P["conv_out"], ksize=3, gn=ops.groupnorm_stats(h, *P["norm_out"]), swish=True, tf32=tf)
+        return ops.conv_nhwc(h, *P["conv_out"], ksize=3, gn=ops.groupnorm_stats(h, *P["norm_out"]), swish=True, tf32=tf)
+
+
+class MVEncoder(_MVEncoderTrunk):
+    """model.py:563-577: the trunk plus a conv fusion of the 4 views of each object (pixel-nerf style)."""
+
+    def __init__(self, *, ch, out_ch, ch_mult=(1, 2, 4, 8), num_res_blocks, attn_resolutions, dropout=0,
+                 resamp_with_conv=True, in_channels, resolution, z_channels, double_z=True, use_linear_attn=False,
+                 attn_type="mv-vanilla", attn_kwargs={}, **ignore_kwargs):
+        super().__init__(ch=ch, out_ch=out_ch, ch_mult=ch_mult, num_res_blocks=num_res_blocks,
+                         attn_resolutions=attn_resolutions, dropout=dropout, resamp_with_conv=resamp_with_conv,
+                         in_channels=in_channels, resolution=resolution, z_channels=z_channels, double_z=double_z,
+                         use_linear_attn=use_linear_attn, attn_type=attn_type, attn_kwargs=attn_kwargs,
+                         add_fusion_layer=True)
+        self.num_frames = 4
+
+    @torch.no_grad()
+    def forward_nhwc(self, x):
+        """x (B*4, in_channels, R, R) fp32 CUDA -> fused moments (B, R/8, R/8, 2*z_channels) NHWC fp32."""
+        F_ = self.num_frames
+        h = self._trunk_nhwc(x, F_)
         N, S, _, Z = h.shape
         # fusion_layer(cat(feat.chunk(F), dim=1)): input channel v*Z + c is channel c of view v
         fused = h.view(N // F_, F_, S, S, Z).permute(0, 2, 3, 1, 4).reshape(N // F_, S, S, F_ * Z)
-        return ops.conv_nhwc(fused, *P["fusion"], ksize=3, tf32=tf)
+        return ops.conv_nhwc(fused, *self._prep["fusion"], ksize=3, tf32=self.conv_tf32)
 
     def forward(self, x):
         """(B*4, in_channels, 256, 256) fp32 -> moments (B, 2*z_channels, 32, 32) fp32, returned as an NCHW view of the
@@ -333,6 +355,51 @@ class MVEncoderGS(nn.Module):
                                   "VAE; only MVEncoder is built")
 
 
-class MVEncoderGSDynamicInp(nn.Module):
-    def __init__(self, *a, **kw):
-        raise NotImplementedError("MVEncoderGSDynamicInp is not part of the release VAE; only MVEncoder is built")
+class MissingArgumentError(NotImplementedError, TypeError):
+    """A required constructor argument is missing.  A TypeError as Python raises for the reference's signature, and a
+    NotImplementedError like the other encoder configurations this package does not build."""
+
+
+_REQUIRED = object()
+
+
+class MVEncoderGSDynamicInp(_MVEncoderTrunk):
+    """model.py:604-623, the encoder of the DiT2-L/2 VAE (dino_version 'mv-sd-dit-dynaInp-trilatent', num_frames 6 in
+    the release scripts): the trunk without a fusion layer, then the mean of the per-view moments over each object's
+    views (ln3_view_mean_nhwc)."""
+
+    def __init__(self, *, ch, out_ch, ch_mult=(1, 2, 4, 8), num_res_blocks, attn_resolutions, dropout=0,
+                 resamp_with_conv=True, in_channels, resolution, z_channels, double_z=True, use_linear_attn=False,
+                 attn_type="mv-vanilla", num_frames=_REQUIRED, **ignore_kwargs):
+        if num_frames is _REQUIRED:
+            raise MissingArgumentError("MVEncoderGSDynamicInp.__init__() missing 1 required keyword-only argument: "
+                                       "'num_frames'")
+        super().__init__(ch=ch, out_ch=out_ch, ch_mult=ch_mult, num_res_blocks=num_res_blocks,
+                         attn_resolutions=attn_resolutions, dropout=dropout, resamp_with_conv=resamp_with_conv,
+                         in_channels=in_channels, resolution=resolution, z_channels=z_channels, double_z=double_z,
+                         use_linear_attn=use_linear_attn, attn_type=attn_type, add_fusion_layer=False, **ignore_kwargs)
+        self.num_frames = num_frames
+
+    @torch.no_grad()
+    def forward_nhwc(self, x, num_frames=None):
+        """x (B*F, in_channels, R, R) fp32 CUDA -> pooled moments (B, R/8, R/8, 2*z_channels) NHWC fp32.  As the
+        reference, the mid-block attention groups the views by self.num_frames whatever `num_frames` is; `num_frames`
+        (default self.num_frames) only sets the pooling: h.chunk(N // num_frames), then the mean of each chunk."""
+        h = self._trunk_nhwc(x, self.num_frames)
+        if num_frames is None:
+            num_frames = self.num_frames
+        assert num_frames > 4
+        N = h.shape[0]
+        if N // num_frames <= 0:
+            raise RuntimeError(f"chunk expects `chunks` to be greater than 0, got: {N // num_frames}")
+        size = -(-N // (N // num_frames))  # torch.chunk: equal chunks of ceil(N / chunks), a shorter last one
+        full = N // size
+        out = ops.view_mean_nhwc(h[:full * size], size)
+        if full * size < N:
+            out = torch.cat([out, ops.view_mean_nhwc(h[full * size:], N - full * size)], 0)
+        return out
+
+    def forward(self, x, num_frames=None):
+        """(B*F, in_channels, 256, 256) fp32 -> moments (B, 2*z_channels, 32, 32) fp32, returned as an NCHW view of the
+        NHWC kernel output (torch.channels_last memory format)."""
+        return self.forward_nhwc(x, num_frames).permute(0, 3, 1, 2)

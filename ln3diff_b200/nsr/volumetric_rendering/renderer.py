@@ -28,8 +28,9 @@ class ImportanceRenderer(torch.nn.Module):
     def _check_options(o):
         if not (o.get("ray_start") == o.get("ray_end") == "auto"):
             raise NotImplementedError("libln3b200 renders the Objaverse preset: ray_start = ray_end = 'auto'")
-        if o.get("depth_resolution") != 64 or o.get("depth_resolution_importance") != 64:
-            raise NotImplementedError("libln3b200 renders 64 coarse + 64 importance samples per ray")
+        S = o.get("depth_resolution")
+        if S not in (64, 96) or o.get("depth_resolution_importance") != S:
+            raise NotImplementedError("libln3b200 renders 64 + 64 or 96 + 96 coarse + importance samples per ray")
         if o.get("disparity_space_sampling", False) or o.get("clamp_mode", "softplus") != "softplus":
             raise NotImplementedError("unsupported sampling / clamp mode")
         if not o.get("filter_out_of_bbox", False):
@@ -68,7 +69,7 @@ class ImportanceRenderer(torch.nn.Module):
                                bbox_min=rendering_options["sampler_bbox_min"],
                                bbox_max=rendering_options["sampler_bbox_max"],
                                white_back=rendering_options.get("white_back", True),
-                               mlp_tf32=rendering_options.get("osg_mlp_tf32", True))
+                               mlp_tf32=rendering_options.get("osg_mlp_tf32", True), samples_per_ray=S)
         depth = out["depth"].permute(0, 2, 1)
         shape_synthesized = {"depth": depth}
         ret = {"feature_samples": out["rgb"].permute(0, 2, 1), "depth_samples": depth,

@@ -694,10 +694,11 @@ def render_views(planes_cl: torch.Tensor, ray_o: torch.Tensor, ray_d: torch.Tens
                  view_obj: torch.Tensor | None = None, views_per_obj: int = 0, group_size: int = 1,
                  box_warp: float = 0.9, bbox_min: float = -0.45, bbox_max: float = 0.45,
                  white_back: bool = True, debug: bool = False, mlp_tf32: bool = False,
-                 image_width: int | None = None):
+                 image_width: int | None = None, samples_per_ray: int = 64):
     """Fused ImportanceRenderer.forward for V views.  Returns dict(rgb (V,3,M), depth (V,1,M),
     weights (V,1,M)) (+ debug index tensors).  mlp_tf32: evaluate the OSG MLP on the tensor cores (TF32
-    operands, fp32 accumulate; pixel error ~1e-4 rel-L2) instead of exact fp32."""
+    operands, fp32 accumulate; pixel error ~1e-4 rel-L2) instead of exact fp32.  samples_per_ray S: the coarse and
+    the importance sample count (64 or 96); the noise tensors hold V*M*S values."""
     for nm, t_ in (("planes_cl", planes_cl), ("ray_o", ray_o), ("ray_d", ray_d),
                    ("noise_coarse", noise_coarse), ("noise_fine", noise_fine)):
         _cuda(t_, nm, torch.float32)
@@ -706,8 +707,10 @@ def render_views(planes_cl: torch.Tensor, ray_o: torch.Tensor, ray_d: torch.Tens
          "planes_cl must be (N,3,H,W,32)")
     V, M, _ = ray_o.shape
     _req(ray_d.shape == (V, M, 3), "ray_d shape")
-    _req(noise_coarse.numel() == V * M * 64 and noise_fine.numel() == V * M * 64,
-         "noise tensors must hold V*M*64 values")
+    S = int(samples_per_ray)
+    _req(S in (64, 96), f"samples_per_ray must be 64 or 96, got {samples_per_ray}")
+    _req(noise_coarse.numel() == V * M * S and noise_fine.numel() == V * M * S,
+         f"noise tensors must hold V*M*{S} values")
     w1, b1, w2, b2 = osg
     for nm, t_, shp in (("w1", w1, (64, 32)), ("b1", b1, (64,)), ("w2", w2, (4, 64)), ("b2", b2, (4,))):
         _cuda(t_, nm, torch.float32)
@@ -731,14 +734,14 @@ def render_views(planes_cl: torch.Tensor, ray_o: torch.Tensor, ray_d: torch.Tens
     a.workspace, a.workspace_bytes = ws.data_ptr(), nbytes
     out = dict(rgb=rgb, depth=depth, weights=wts)
     if debug:
-        out["inbox"] = torch.empty((V * M, 128), device=dev, dtype=torch.uint8)
-        out["inds"] = torch.empty((V * M, 64), device=dev, dtype=torch.int32)
-        out["order"] = torch.empty((V * M, 128), device=dev, dtype=torch.int32)
-        out["z_fine"] = torch.empty((V * M, 64), device=dev, dtype=torch.float32)
+        out["inbox"] = torch.empty((V * M, 2 * S), device=dev, dtype=torch.uint8)
+        out["inds"] = torch.empty((V * M, S), device=dev, dtype=torch.int32)
+        out["order"] = torch.empty((V * M, 2 * S), device=dev, dtype=torch.int32)
+        out["z_fine"] = torch.empty((V * M, S), device=dev, dtype=torch.float32)
         a.dbg_inbox, a.dbg_inds = out["inbox"].data_ptr(), out["inds"].data_ptr()
         a.dbg_order, a.dbg_zfine = out["order"].data_ptr(), out["z_fine"].data_ptr()
     a.V, a.M, a.H, a.W, a.C = V, M, planes_cl.shape[2], planes_cl.shape[3], 32
-    a.S, a.S_importance, a.hidden_dim, a.decoder_output_dim = 64, 64, 64, 3
+    a.S, a.S_importance, a.hidden_dim, a.decoder_output_dim = S, S, 64, 3
     a.group_size, a.views_per_obj, a.white_back = group_size, views_per_obj, int(white_back)
     a.box_warp, a.bbox_min, a.bbox_max = box_warp, bbox_min, bbox_max
     a.mlp_precision = _lib.MLP_TF32 if mlp_tf32 else _lib.MLP_FP32
@@ -890,6 +893,19 @@ def vae_posterior(moments: torch.Tensor, w: torch.Tensor, bias: torch.Tensor, no
     a.mean, a.logvar, a.z, a.B, a.S = mean.data_ptr(), logvar.data_ptr(), z.data_ptr(), B, S
     _lib.check(_lib.lib().ln3_vae_posterior(C.byref(a), _lib.current_stream()), "ln3_vae_posterior")
     return mean, logvar, z
+
+
+def view_mean_nhwc(x: torch.Tensor, num_frames: int) -> torch.Tensor:
+    """x (B*F, S, S, C) NHWC fp32 -> (B, S, S, C): the mean over each object's F = num_frames consecutive views."""
+    _cuda(x, "x", torch.float32)
+    _req(x.dim() == 4 and x.shape[1] == x.shape[2] and x.is_contiguous(), "x must be contiguous (N,S,S,C)")
+    F_ = int(num_frames)
+    _req(F_ > 0 and x.shape[0] % F_ == 0, f"x holds {x.shape[0]} views, not a multiple of num_frames={num_frames}")
+    N, S, _, Cc = x.shape
+    out = torch.empty((N // F_, S, S, Cc), device=x.device, dtype=torch.float32)
+    _lib.check(_lib.lib().ln3_view_mean_nhwc(_lib.ptr(x), _lib.ptr(out), N // F_, F_, S, Cc, _lib.current_stream()),
+               "ln3_view_mean_nhwc")
+    return out
 
 
 def groupnorm_stats(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, groups: int = 32,

@@ -278,8 +278,9 @@ def decode_and_render(decoder, latents: torch.Tensor, cameras: torch.Tensor, res
     decodes twice, :204-206 and :268-270) -> every camera of `cameras` (V,25) for every latent in
     fused renderer launches.  Per-view global reductions (group_size=1) reproduce the reference's
     one-view-per-call loop (:292-302).  Returns image_raw (B,V,3,H,W) in [-1,1], image_depth
-    (B,V,1,H,W), image_mask (B,V,1,H,W).  `noise` = (coarse, fine) tensors of shape (B*V, H*W, 64) to
-    override the device RNG (tests).  The sampling noise costs 512 B per ray, so the views are rendered in
+    (B,V,1,H,W), image_mask (B,V,1,H,W).  The samples per ray S (coarse = importance, 64 or 96) come from
+    decoder.rendering_kwargs['depth_resolution'].  `noise` = (coarse, fine) tensors of shape (B*V, H*W, S) to
+    override the device RNG (tests).  The sampling noise costs 8*S bytes per ray, so the views are rendered in
     launches of whole objects with at most `max_views_per_launch` views (default: ~2 GiB of noise)."""
     if not latents.is_cuda:
         raise RuntimeError("decode_and_render runs on CUDA only (no CPU fallback)")
@@ -290,10 +291,11 @@ def decode_and_render(decoder, latents: torch.Tensor, cameras: torch.Tensor, res
     planes_cl = decoder.decode_to_channels_last(latents, in_mul=scaling_divider)     # (B,3,128,128,32)
     cams1 = cameras.to(dev, torch.float32).contiguous()                               # (V, 25)
     ray_o1, ray_d1 = ops.generate_rays(cams1, resolution)                              # shared by every object
-    if max_views_per_launch is None:
-        max_views_per_launch = max(V, (2 << 30) // (2 * M * 64 * 4))
-    obj_per_launch = max(1, min(B, max_views_per_launch // V))
     kw = decoder.rendering_kwargs
+    S = kw.get("depth_resolution", 64)
+    if max_views_per_launch is None:
+        max_views_per_launch = max(V, (2 << 30) // (2 * M * S * 4))
+    obj_per_launch = max(1, min(B, max_views_per_launch // V))
     osg = decoder.triplane_decoder.decoder.raw_parameters()
     rgb = torch.empty(B, V, 3, H, W, device=dev)
     depth = torch.empty(B, V, 1, H, W, device=dev)
@@ -301,14 +303,14 @@ def decode_and_render(decoder, latents: torch.Tensor, cameras: torch.Tensor, res
     for b0 in range(0, B, obj_per_launch):
         nb = min(obj_per_launch, B - b0)
         if noise is None:
-            nz = (torch.rand(nb * V, M, 64, device=dev), torch.rand(nb * V, M, 64, device=dev))
+            nz = (torch.rand(nb * V, M, S, device=dev), torch.rand(nb * V, M, S, device=dev))
         else:
             nz = (noise[0][b0 * V:(b0 + nb) * V].contiguous(), noise[1][b0 * V:(b0 + nb) * V].contiguous())
         out = ops.render_views(planes_cl[b0:b0 + nb], ray_o1.repeat(nb, 1, 1), ray_d1.repeat(nb, 1, 1), nz[0], nz[1],
                                osg, views_per_obj=V, group_size=1,
                                box_warp=kw.get("box_warp", 0.9), bbox_min=kw.get("sampler_bbox_min", -0.45),
                                bbox_max=kw.get("sampler_bbox_max", 0.45), white_back=kw.get("white_back", True),
-                               mlp_tf32=mlp_tf32)
+                               mlp_tf32=mlp_tf32, samples_per_ray=S)
         rgb[b0:b0 + nb].copy_(out["rgb"].view(nb, V, 3, H, W))
         depth[b0:b0 + nb].copy_(out["depth"].view(nb, V, 1, H, W))
         wts[b0:b0 + nb].copy_(out["weights"].view(nb, V, 1, H, W))
@@ -538,9 +540,10 @@ def image_to_3d(conditioner, model, decoder, image: torch.Tensor, cameras: torch
 @torch.no_grad()
 def encode_latents(encoder, decoder, img_to_encoder: torch.Tensor, sample_posterior: bool = True) -> dict:
     """`AE.forward(img=img_to_encoder, behaviour='encoder_vae')` (nsr/script_util.py:326-329), the first step of
-    `eval_novelview_loop` (nsr/train_nv_util.py:1177-1219): img_to_encoder (B*4, 10, 256, 256) fp32 -- per view RGB in
-    [-1, 1], the Plücker rays o x d and d, and depth -- through MVEncoder to the moments (B, 24, 32, 32), then the
-    decoder's vae_reparameterization.  Returns the reference's dict; `latent_normalized_2Ddiffusion` (B, 12, 32, 32) is
+    `eval_novelview_loop` (nsr/train_nv_util.py:1177-1219): img_to_encoder (B*F, 10, 256, 256) fp32 with
+    F = encoder.num_frames views per object (4 for MVEncoder, 6 for the DiT2-L/2 VAE's MVEncoderGSDynamicInp) -- per
+    view RGB in [-1, 1], the Plücker rays o x d and d, and depth -- through the encoder to the moments (B, 24, 32, 32),
+    then the decoder's vae_reparameterization.  Returns the reference's dict; `latent_normalized_2Ddiffusion` (B, 12, 32, 32) is
     the latent every stage-2 DiT is trained on (what `--save_latent True` writes).  sample_posterior draws the noise
     from the CPU generator, as the reference does."""
     if not img_to_encoder.is_cuda:
@@ -552,8 +555,9 @@ def encode_latents(encoder, decoder, img_to_encoder: torch.Tensor, sample_poster
 def reconstruct(encoder, decoder, img_to_encoder: torch.Tensor, cameras: torch.Tensor, resolution: int = 128,
                 scaling_divider: float = 1.0, sample_posterior: bool = True, noise: tuple | None = None,
                 mlp_tf32: bool = True):
-    """3D reconstruction from multi-view images, the body of `eval_novelview_loop`: `encode_latents`, then decode and
-    render of every camera of `cameras` (V, 25) for every object.  The reconstruction trainer renders the posterior
+    """3D reconstruction from multi-view images, the body of `eval_novelview_loop`: `encode_latents` of img_to_encoder
+    (B*F, 10, 256, 256), F = encoder.num_frames, then decode and render of every camera of `cameras` (V, 25) for every
+    object at the decoder's samples per ray.  The reconstruction trainer renders the posterior
     latent with `triplane_scaling_divider = 1.0` (TrainLoop3DRec, nsr/train_util.py:565, applied at :580).
     Returns (the encoder_vae dict, the render dict of `decode_and_render`)."""
     ret = encode_latents(encoder, decoder, img_to_encoder, sample_posterior)

@@ -112,9 +112,12 @@ OBJAVERSE_RENDERING_KWARGS = dict(  # nsr/script_util.py:433-465,761-797 (resolv
     z_near=1.05, z_far=2.45)
 
 
-def build_ae_decoder(arch: str = "DiT2-L/2", image_size: int = 128, seed: int = 0, device: str | None = None):
+def build_ae_decoder(arch: str = "DiT2-L/2", image_size: int = 128, seed: int = 0, device: str | None = None,
+                     depth_resolution: int = 64):
     """The AE decoder as create_3DAE_model assembles it for the Objaverse release
-    (nsr/script_util.py:1355-1429): Triplane renderer + DiT2 backbone + SD conv upsampler."""
+    (nsr/script_util.py:1355-1429): Triplane renderer + DiT2 backbone + SD conv upsampler.  depth_resolution sets
+    the coarse and the importance samples per ray: 64 (objaverse_tuneray_aug_resolution_64_64_auto) or 96 (the
+    96_96 preset of the DiT2-L/2 VAE's reconstruction script, nsr/script_util.py:838-870)."""
     from .dit.dit_decoder import DiT2_models
     from .nsr.triplane import Triplane
     from .vit.vit_triplane import (
@@ -124,7 +127,9 @@ def build_ae_decoder(arch: str = "DiT2-L/2", image_size: int = 128, seed: int = 
     vd = DiT2_models[arch](input_size=16, num_classes=0, learn_sigma=False, in_channels=D, mixed_prediction=False,
                            context_dim=None, roll_out=True, plane_n=3, return_all_layers=False)
     tri = Triplane(c_dim=25, img_resolution=image_size, img_channels=3, out_chans=96, triplane_size=224,
-                   rendering_kwargs=dict(OBJAVERSE_RENDERING_KWARGS), decoder_in_chans=32, decoder_output_dim=3)
+                   rendering_kwargs=dict(OBJAVERSE_RENDERING_KWARGS, depth_resolution=depth_resolution,
+                                         depth_resolution_importance=depth_resolution),
+                   decoder_in_chans=32, decoder_output_dim=3)
     m = AEDec(vd, tri, False, vae_p=2, ldm_z_channels=4, ldm_embed_dim=4)
     derandomize_zero_init(m)
     m.eval()
@@ -132,17 +137,24 @@ def build_ae_decoder(arch: str = "DiT2-L/2", image_size: int = 128, seed: int = 
 
 
 def build_ae_encoder(seed: int = 0, device: str | None = None, ch: int = 64, num_res_blocks: int = 1,
-                     in_channels: int = 10):
-    """The stage-1 encoder as create_3DAE_model builds it for dino_version 'mv-sd-dit' (nsr/script_util.py:1294-1339)
-    with the release scripts' sd_E_ch=64, sd_E_num_res_blocks=1: MVEncoder(double_z=True, resolution=256,
-    in_channels=10, ch_mult=[1,2,4,4], z_channels=12, attn_kwargs={'n_heads': 8, 'd_head': 64}).  Random init; the
-    zero-initialised proj_out of the mid-block transformer is re-randomised (derandomize_zero_init), otherwise the
-    whole transformer would be multiplied by zero."""
-    from .ldm.modules.diffusionmodules.model import MVEncoder
+                     in_channels: int = 10, dino_version: str = "mv-sd-dit", num_frames: int | None = None):
+    """The stage-1 encoder as create_3DAE_model builds it (nsr/script_util.py:1294-1339) with the release scripts'
+    sd_E_ch=64, sd_E_num_res_blocks=1: encoder_cls(double_z=True, resolution=256, in_channels=10, ch_mult=[1,2,4,4],
+    z_channels=12, attn_kwargs={'n_heads': 8, 'd_head': 64}).  encoder_cls is MVEncoder for dino_version 'mv-sd-dit'
+    (4 views) and MVEncoderGSDynamicInp for 'mv-sd-dit-dynaInp-trilatent' (the DiT2-L/2 VAE; num_frames defaults to
+    the release scripts' 6).  Random init; the zero-initialised proj_out of the mid-block transformer is re-randomised
+    (derandomize_zero_init), otherwise the whole transformer would be multiplied by zero."""
+    from .ldm.modules.diffusionmodules.model import MVEncoder, MVEncoderGSDynamicInp
+    if dino_version == "mv-sd-dit":
+        cls, num_frames = MVEncoder, 4 if num_frames is None else num_frames
+    elif dino_version == "mv-sd-dit-dynaInp-trilatent":
+        cls, num_frames = MVEncoderGSDynamicInp, 6 if num_frames is None else num_frames
+    else:
+        raise NotImplementedError(f"dino_version {dino_version!r}: only the release VAE encoders are built")
     torch.manual_seed(seed)
-    m = MVEncoder(double_z=True, resolution=256, in_channels=in_channels, ch=ch, ch_mult=[1, 2, 4, 4],
-                  num_res_blocks=num_res_blocks, num_frames=4, dropout=0.0, attn_resolutions=[], out_ch=3,
-                  z_channels=12, attn_kwargs={"n_heads": 8, "d_head": 64})
+    m = cls(double_z=True, resolution=256, in_channels=in_channels, ch=ch, ch_mult=[1, 2, 4, 4],
+            num_res_blocks=num_res_blocks, num_frames=num_frames, dropout=0.0, attn_resolutions=[], out_ch=3,
+            z_channels=12, attn_kwargs={"n_heads": 8, "d_head": 64})
     derandomize_zero_init(m)
     m.eval()
     return m.to(device) if device else m
