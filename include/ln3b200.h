@@ -321,6 +321,48 @@ typedef struct ln3_sampler_step_args {
 
 int ln3_sampler_step(const ln3_sampler_step_args* args, void* stream);
 
+/* ------------------------------------------------------------------ flow-matching SDE step
+ * The elementwise tail of one drift evaluation of the transport's SDE samplers (transport/integrators.py:9-75,
+ * transport/transport.py:246-372, path.py:18-110: Euler-Maruyama and Heun on the Linear path with velocity
+ * prediction) around a CFG denoiser.  The state has 2R rows of n elements: rows [0, R) are the conditional half,
+ * [R, 2R) the unconditional half, R = P * N condition-major (P conditions of N samples).  The two halves diverge
+ * (each row draws its own noise), but both move under the same guided velocity.  For state row r, j = r mod R:
+ *   v   = f[R+j] + s * (f[j] - f[R+j])       guided velocity (f: the forward output, conditional rows first)
+ *   sc  = (t * v - y[r]) / var               score at the evaluated input y (var = sigma_t^2 + t sigma_t)
+ *   d   = v + D * sc (LN3_SDE_DRIFT) | v (LN3_SDE_VELOCITY) | sc (LN3_SDE_SCORE)
+ *   o(k) = k[0] * x[r] + k[1] * y[r] + k[2] * d + k[3] * hist[r] + k[4] * w[noise_row(r)]
+ *   x_out[r] = o(cx);  y_out[r] = o(cy);  hist_out[r] = d
+ * v, sc and d are rounded as the reference's separate fp32 tensor ops (no contraction); o is one fmaf chain, left
+ * to right.  Each output has its own coefficients, so the state can be written without the noise term while the
+ * next forward's input gets it.  noise_row(r) = (r < R ? 0 : N) + (j mod N): w is one (2N, n) draw whose rows
+ * [0, N) serve the conditional half and [N, 2N) the unconditional half of every condition, as P sequential
+ * samplers seeded alike would draw.  A NULL x, hist or noise drops its term; a NULL output is not written.
+ * R >= 0; n % 4 == 0; y and f non-NULL; at least one output; mode one of LN3_SDE_*; with noise, 0 < N <= R and
+ * R % N == 0; every non-NULL pointer 16-byte aligned.  x, y, f, hist and every output hold 2R rows, noise 2N.
+ * No output may overlap another output or an input, except x_out == x and y_out == y (same start: the element is
+ * read before it is written by the same thread).  LN3_EINVAL otherwise, before any CUDA call.
+ */
+enum { LN3_SDE_DRIFT = 0, LN3_SDE_VELOCITY = 1, LN3_SDE_SCORE = 2 };
+
+typedef struct ln3_flow_sde_step_args {
+  const float* x;       /* [2R, n] state (optional) */
+  const float* y;       /* [2R, n] the evaluated input */
+  const float* f;       /* [2R, n] forward output at y */
+  const float* hist;    /* [2R, n] optional */
+  const float* noise;   /* [2N, n] optional */
+  float* x_out;
+  float* y_out;
+  float* hist_out;
+  float cx[5];          /* x_out: (a, b, c, h, sigma) */
+  float cy[5];          /* y_out: (a, b, c, h, sigma) */
+  float cfg_scale, t, var, diffusion;
+  int mode;
+  int R, N;
+  long long n;
+} ln3_flow_sde_step_args;
+
+int ln3_flow_sde_step(const ln3_flow_sde_step_args* args, void* stream);
+
 /* ------------------------------------------------------------------ grouped adaptive dopri5
  * The per-attempt arithmetic of the adaptive Dormand-Prince 5(4) solver that `sample_ode`'s default runs
  * (transport/transport.py:374-421 -> transport/integrators.py:101-120 -> torchdiffeq odeint(method='dopri5')),

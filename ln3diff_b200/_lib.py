@@ -125,6 +125,16 @@ class SamplerStepArgs(C.Structure):
     ]
 
 
+class FlowSdeStepArgs(C.Structure):
+    _fields_ = [
+        ("x", C.c_void_p), ("y", C.c_void_p), ("f", C.c_void_p), ("hist", C.c_void_p), ("noise", C.c_void_p),
+        ("x_out", C.c_void_p), ("y_out", C.c_void_p), ("hist_out", C.c_void_p),
+        ("cx", C.c_float * 5), ("cy", C.c_float * 5),
+        ("cfg_scale", C.c_float), ("t", C.c_float), ("var", C.c_float), ("diffusion", C.c_float),
+        ("mode", C.c_int), ("R", C.c_int), ("N", C.c_int), ("n", C.c_longlong),
+    ]
+
+
 class RenderArgs(C.Structure):
     _fields_ = [
         ("planes_cl", C.c_void_p), ("view_obj", C.c_void_p), ("ray_o", C.c_void_p),

@@ -207,6 +207,49 @@ static int sampler_step_validate(const ln3_sampler_step_args* a) {
   return LN3_OK;
 }
 
+// The rules of ln3_flow_sde_step (include/ln3b200.h): sizes, mode, NULLs, the noise row mapping, alignment, and no
+// output range overlapping another output or an input except the in-place updates x_out == x and y_out == y.
+static int flow_sde_step_validate(const ln3_flow_sde_step_args* a) {
+  if (!a) return set_error(LN3_EINVAL, "flow_sde_step: null args");
+  if (a->R < 0 || a->n < 0) return set_error(LN3_EINVAL, "flow_sde_step: negative R or n");
+  if (a->R > 32767) return set_error(LN3_EINVAL, "flow_sde_step: R > 32767 (2R rows are one grid dimension)");
+  if (a->n % 4) return set_error(LN3_EINVAL, "flow_sde_step: n % 4 != 0");
+  if (a->R > 0 && a->n > (1ll << 50) / (8ll * a->R)) return set_error(LN3_EINVAL, "flow_sde_step: R * n too large");
+  if (a->mode != LN3_SDE_DRIFT && a->mode != LN3_SDE_VELOCITY && a->mode != LN3_SDE_SCORE)
+    return set_error(LN3_EINVAL, "flow_sde_step: unknown mode %d", a->mode);
+  if (!a->y || !a->f) return set_error(LN3_EINVAL, "flow_sde_step: null y or f");
+  if (!a->x_out && !a->y_out && !a->hist_out) return set_error(LN3_EINVAL, "flow_sde_step: no output");
+  if (a->noise && (a->N <= 0 || a->N > a->R || a->R % a->N))
+    return set_error(LN3_EINVAL, "flow_sde_step: noise rows need 0 < N <= R and R %% N == 0 (N = %d, R = %d)", a->N,
+                     a->R);
+  struct Range { const char* name; const void* p; unsigned long long bytes; };
+  const unsigned long long rows = 8ull * static_cast<unsigned long long>(a->R) * a->n;   // 2R rows of fp32
+  const unsigned long long nrows = a->noise ? 8ull * static_cast<unsigned long long>(a->N) * a->n : 0;
+  const Range in[] = {{"x", a->x, rows}, {"y", a->y, rows}, {"f", a->f, rows}, {"hist", a->hist, rows},
+                      {"noise", a->noise, nrows}};
+  const Range out[] = {{"x_out", a->x_out, rows}, {"y_out", a->y_out, rows}, {"hist_out", a->hist_out, rows}};
+  for (const Range& r : in)
+    if (misaligned16(r.p)) return set_error(LN3_EINVAL, "flow_sde_step: %s must be 16-byte aligned", r.name);
+  for (const Range& r : out)
+    if (misaligned16(r.p)) return set_error(LN3_EINVAL, "flow_sde_step: %s must be 16-byte aligned", r.name);
+  auto overlap = [](const Range& u, const Range& v) {
+    if (!u.p || !v.p || u.bytes == 0 || v.bytes == 0) return false;
+    const uintptr_t a0 = reinterpret_cast<uintptr_t>(u.p), b0 = reinterpret_cast<uintptr_t>(v.p);
+    return a0 < b0 + v.bytes && b0 < a0 + u.bytes;
+  };
+  for (int i = 0; i < 3; ++i) {
+    for (int j = i + 1; j < 3; ++j)
+      if (overlap(out[i], out[j]))
+        return set_error(LN3_EINVAL, "flow_sde_step: outputs %s and %s overlap", out[i].name, out[j].name);
+    for (int j = 0; j < 5; ++j) {
+      const bool alias = out[i].p == in[j].p && ((i == 0 && j == 0) || (i == 1 && j == 1));
+      if (!alias && overlap(out[i], in[j]))
+        return set_error(LN3_EINVAL, "flow_sde_step: output %s overlaps input %s", out[i].name, in[j].name);
+    }
+  }
+  return LN3_OK;
+}
+
 }  // namespace ln3
 
 using namespace ln3;
@@ -256,6 +299,11 @@ int ln3_sampler_step(const ln3_sampler_step_args* args, void* stream) {
   const int rc = sampler_step_validate(args);
   if (rc != LN3_OK) return rc;
   return sampler_step(args, static_cast<cudaStream_t>(stream));
+}
+int ln3_flow_sde_step(const ln3_flow_sde_step_args* args, void* stream) {
+  const int rc = flow_sde_step_validate(args);
+  if (rc != LN3_OK) return rc;
+  return flow_sde_step(args, static_cast<cudaStream_t>(stream));
 }
 
 size_t ln3_render_workspace_bytes(int V, int M, int group_size) {

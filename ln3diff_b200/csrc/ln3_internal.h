@@ -84,6 +84,7 @@ int plucker_patchify(const ln3_plucker_patchify_args* a, cudaStream_t stream);
 int final_layer(const ln3_final_layer_args* a, cudaStream_t stream);
 int sampler_affine_update(const ln3_sampler_update_args* a, cudaStream_t stream);
 int sampler_step(const ln3_sampler_step_args* a, cudaStream_t stream);   // arguments validated by the caller
+int flow_sde_step(const ln3_flow_sde_step_args* a, cudaStream_t stream);   // arguments validated by the caller
 size_t render_workspace_bytes(int V, int M, int group_size);
 int render_tile_width(int M, int image_w);
 int render_views(const ln3_render_args* a, cudaStream_t stream);

@@ -529,6 +529,54 @@ def sampler_step(x: torch.Tensor, x_eval: torch.Tensor, coef: torch.Tensor, net_
     _lib.check(_lib.lib().ln3_sampler_step(C.byref(a), _lib.current_stream()), "ln3_sampler_step")
 
 
+SDE_DRIFT, SDE_VELOCITY, SDE_SCORE = 0, 1, 2   # LN3_SDE_*: d = v + D sc | v | sc
+
+
+def flow_sde_step(y: torch.Tensor, f: torch.Tensor, *, cfg_scale: float, t: float, var: float,
+                  diffusion: float = 0.0, mode: int = SDE_DRIFT, x: torch.Tensor | None = None,
+                  hist: torch.Tensor | None = None, noise: torch.Tensor | None = None,
+                  x_out: torch.Tensor | None = None, cx=(0.0,) * 5, y_out: torch.Tensor | None = None,
+                  cy=(0.0,) * 5, hist_out: torch.Tensor | None = None) -> None:
+    """One drift evaluation's elementwise tail of the flow SDE samplers (include/ln3b200.h, ln3_flow_sde_step_args)
+    over the 2R-row CFG state (conditional rows first), per row r and j = r mod R:
+        v = f[R+j] + s (f[j] - f[R+j]);  sc = (t v - y[r]) / var;  d = v + D sc | v | sc  (mode)
+        o(k) = k0 x[r] + k1 y[r] + k2 d + k3 hist[r] + k4 noise[noise_row(r)]
+        x_out[r] = o(cx);  y_out[r] = o(cy);  hist_out[r] = d
+    `noise` is one (2N, ...) draw: rows [0, N) serve the conditional half and [N, 2N) the unconditional half of
+    every one of the R / N conditions.  Every tensor is CUDA fp32, contiguous and 16-byte aligned, with 2R rows of n
+    elements (n % 4 == 0).  Outputs are written in place; at least one is required.  No output may overlap another
+    output or an input, except x_out is x and y_out is y (checked by the library)."""
+    _cuda(y, "y", torch.float32)
+    _req(y.dim() >= 1 and y.shape[0] % 2 == 0, "y must hold 2R rows")
+    R2 = y.shape[0]
+    n = y[0].numel() if R2 else 0
+    _req(n % 4 == 0, "elements per row must be a multiple of 4")
+    _req(mode in (SDE_DRIFT, SDE_VELOCITY, SDE_SCORE), f"unknown mode {mode}")
+    _req(any(o is not None for o in (x_out, y_out, hist_out)), "at least one of x_out, y_out, hist_out is required")
+    N = 0
+    if noise is not None:
+        _req(noise.dim() >= 1 and noise.shape[0] % 2 == 0, "noise must hold 2N rows")
+        N = noise.shape[0] // 2
+    for nm, t_, rows in (("y", y, R2), ("f", f, R2), ("x", x, R2), ("hist", hist, R2), ("noise", noise, 2 * N),
+                         ("x_out", x_out, R2), ("y_out", y_out, R2), ("hist_out", hist_out, R2)):
+        if t_ is None:
+            continue
+        _cuda(t_, nm, torch.float32)
+        _req(t_.is_contiguous() and t_.shape[0] == rows and t_.numel() == rows * n,
+             f"{nm} must be contiguous with {rows} rows of {n} elements")
+        _req(t_.data_ptr() % 16 == 0, f"{nm} must be 16-byte aligned (the kernel uses 128-bit accesses)")
+    _req(len(cx) == 5 and len(cy) == 5, "cx and cy hold (a, b, c, h, sigma)")
+    a = _lib.FlowSdeStepArgs()
+    ptr = lambda t_: t_.data_ptr() if t_ is not None else None
+    a.x, a.y, a.f, a.hist, a.noise = ptr(x), y.data_ptr(), f.data_ptr(), ptr(hist), ptr(noise)
+    a.x_out, a.y_out, a.hist_out = ptr(x_out), ptr(y_out), ptr(hist_out)
+    for k in range(5):
+        a.cx[k], a.cy[k] = float(cx[k]), float(cy[k])
+    a.cfg_scale, a.t, a.var, a.diffusion = float(cfg_scale), float(t), float(var), float(diffusion)
+    a.mode, a.R, a.N, a.n = int(mode), R2 // 2, N, n
+    _lib.check(_lib.lib().ln3_flow_sde_step(C.byref(a), _lib.current_stream()), "ln3_flow_sde_step")
+
+
 # ---------------------------------------------------------------------------------------------- grouped dopri5
 ODE_GROUP_BYTES = C.sizeof(_lib.OdeGroup)
 _ODE_F64 = ("t", "dt", "t_prev", "dt_step", "ratio", "aux")

@@ -362,7 +362,8 @@ def text_to_3d(conditioner, model, decoder, prompt, cameras, num_samples: int = 
 
 @torch.no_grad()
 def sample_flow(model, c: dict, uc: dict, num_samples: int, seed: int = 42, num_steps: int = 250,
-                cfg_scale: float = 4.0, sampling_method: str = "dopri5", dtype=torch.float32) -> torch.Tensor:
+                cfg_scale: float = 4.0, sampling_method: str = "dopri5", dtype=torch.float32,
+                sde: dict | None = None) -> torch.Tensor:
     """`FlowMatchingEngine.sample` (nsr/lsgm/flow_matching_trainer.py:509-551) for the image-conditioned denoisers
     (I23D 'img', MV23D 'img-c'): global `torch.manual_seed(seed)` -- which also seeds the CUDA generators that the
     renderer's noise draws use afterwards -- then a CPU `randn(num_samples, 12, 32, 32)`, the CFG batch
@@ -372,11 +373,14 @@ def sample_flow(model, c: dict, uc: dict, num_samples: int, seed: int = 42, num_
     Engine dtype: as on the existing I23D path, the ODE state and the context are carried in fp32 and the denoiser
     rounds its GEMM operands to bf16 itself.  The engine's `.to(self.dtype)` casts of the noise and the context
     (bf16 under `use_amp`) are applied as roundings to `dtype`; the default float32 leaves them exact.
+
+    `sde`: a dict of `sample_sde` keywords samples with the SDE instead of the ODE (see `sample_flow_sde`).
     Returns the denoised latents (num_samples, 12, 32, 32) fp32."""
     from .transport import Sampler, create_transport
     dev = next(model.parameters()).device
     if dev.type != "cuda":
         raise RuntimeError("sample_flow runs on CUDA only (no CPU fallback)")
+    _check_sde_method(sde, sampling_method)
     torch.manual_seed(seed)
     C = 3 * model.in_channels if model.roll_out else model.in_channels
     zs = torch.randn(num_samples, C, model.input_size, model.input_size).to(dev).to(dtype).float()
@@ -387,9 +391,72 @@ def sample_flow(model, c: dict, uc: dict, num_samples: int, seed: int = 42, num_
         else:
             assert c[k] == uc[k]
             ctx[k] = c[k]
+    if sde is not None:
+        return sample_flow_sde(model, zs, ctx, num_samples, num_steps, cfg_scale, sde)[0][:num_samples]
     fn = Sampler(create_transport(snr_type="lognorm")).sample_ode(sampling_method=sampling_method, num_steps=num_steps)
     samples = fn(torch.cat([zs, zs], 0), model.forward_with_cfg, context=ctx, cfg_scale=cfg_scale)[-1]
     return samples.chunk(2, dim=0)[0]
+
+
+# ---------------------------------------------------------------------------------------------- flow SDE
+# parse_sde_args' defaults (transport/train_utils.py:23-33); num_steps comes from the sampling function.
+SDE_DEFAULTS = dict(sampling_method="Euler", diffusion_form="sigma", diffusion_norm=1.0, last_step="Mean",
+                    last_step_size=0.04)
+
+
+def sde_options(sde: dict) -> dict:
+    """`sde=` of the flow pipelines completed with SDE_DEFAULTS."""
+    unknown = set(sde) - set(SDE_DEFAULTS)
+    if unknown:
+        raise ValueError(f"sde= takes the sample_sde keywords {sorted(SDE_DEFAULTS)} (num_steps comes from the "
+                         f"function), got {sorted(unknown)}")
+    return {**SDE_DEFAULTS, **sde}
+
+
+def _check_sde_method(sde, sampling_method):
+    if sde is not None and sampling_method != "dopri5":
+        raise ValueError(f"sampling_method={sampling_method!r} selects an ODE solver; with sde= the SDE method is "
+                         "sde['sampling_method']")
+
+
+class _PinnedNoise:
+    """Step noise on the global CPU generator, `randn(shape)` per call as the reference draws it, moved to the device
+    through a ring of pinned buffers and non-blocking copies: the host waits only for the copy made `depth` draws
+    earlier, never for the stream.  Returns one device buffer that every call overwrites in stream order."""
+
+    def __init__(self, shape, device, depth: int = 3):
+        self.host = [torch.empty(shape).pin_memory() for _ in range(depth)]
+        self.copied = [None] * depth
+        self.dev = torch.empty(shape, device=device)
+        self.k = 0
+
+    def __call__(self, step: int) -> torch.Tensor:
+        i = self.k % len(self.host)
+        self.k += 1
+        if self.copied[i] is not None:
+            self.copied[i].synchronize()
+        torch.randn(self.host[i].shape, out=self.host[i])
+        self.dev.copy_(self.host[i], non_blocking=True)
+        self.copied[i] = torch.cuda.Event()
+        self.copied[i].record()
+        return self.dev
+
+
+@torch.no_grad()
+def sample_flow_sde(model, zs: torch.Tensor, ctx: dict, num_samples: int, num_steps: int, cfg_scale: float,
+                    sde: dict):
+    """`Sampler(create_transport(snr_type='lognorm')).sample_sde(**sde, num_steps=num_steps)` on cat([zs, zs]) around
+    `model.forward_with_cfg`, keeping only the running state (transport/transport.py:sde_fused): per drift evaluation
+    one forward of the 2R-row CFG batch (a CUDA-graph replay) and one ln3_flow_sde_step.  zs (R, ...) CUDA fp32 holds
+    R / num_samples conditions of num_samples rows; ctx is the CFG context cat((c, uc)).  Each step draws the
+    reference's randn(2 * num_samples, ...) on the global CPU generator, which every condition shares.
+    Returns (final state (2R, ...), the evaluation plan)."""
+    from .transport.transport import sde_fused, sde_plan
+    o = sde_options(sde)
+    plan = sde_plan(o["sampling_method"], o["diffusion_form"], o["diffusion_norm"], o["last_step"],
+                    o["last_step_size"], num_steps)
+    draw = _PinnedNoise((2 * num_samples,) + tuple(zs.shape[1:]), zs.device)
+    return sde_fused(plan, model, torch.cat([zs, zs], 0), ctx, cfg_scale, draw), plan
 
 
 def flow_batch_row_groups(P: int, num_samples: int) -> torch.Tensor:
@@ -423,7 +490,7 @@ def flow_batch_context(c: dict, uc: dict, dev=None, dtype=torch.float32) -> dict
 
 @torch.no_grad()
 def sample_flow_batched(model, c: dict, uc: dict, num_samples: int, seed: int = 42, num_steps: int = 250,
-                        cfg_scale: float = 4.0, dtype=torch.float32):
+                        cfg_scale: float = 4.0, dtype=torch.float32, sde: dict | None = None):
     """`sample_flow` with its default dopri5 solver for P conditions in one denoiser batch.  c / uc hold P conditions
     stacked condition-major, each repeated `num_samples` times as `condition_prompt` returns it ((P*N, ...) per key).
     The batch is cat([zs, zs]) of 2PN rows with context cat((c, uc)); every condition runs its own adaptive dopri5
@@ -431,7 +498,12 @@ def sample_flow_batched(model, c: dict, uc: dict, num_samples: int, seed: int = 
     the batch.  The noise is `flow_batch_noise` (sample_flow's draw for every condition).  num_steps is the output
     grid of sample_ode; dopri5 only uses its last point, t = 1.
     Returns (latents (P, N, 12, 32, 32) fp32, stats) with per-condition lists nfe / accepted / rejected and the
-    batch's forward count batch_nfe."""
+    batch's forward count batch_nfe.
+
+    With `sde` (a dict of `sample_sde` keywords, see `sample_flow_sde`) the P conditions instead run the SDE on the
+    shared fixed grid of num_steps points; every condition reads the noise draw its own `sample_flow(..., sde=)` call
+    would make, so its latents are that call's up to the rounding of the batched GEMMs.  stats then hold nfe (per
+    condition) and batch_nfe, both the forward count."""
     from .transport.dopri5 import odeint_dopri5_grouped
     dev = next(model.parameters()).device
     if dev.type != "cuda":
@@ -444,6 +516,9 @@ def sample_flow_batched(model, c: dict, uc: dict, num_samples: int, seed: int = 
     shape = (C, model.input_size, model.input_size)
     zs = flow_batch_noise(P, N, shape, seed).to(dev).to(dtype).float()
     ctx = flow_batch_context(c, uc, dev, dtype)
+    if sde is not None:
+        x, plan = sample_flow_sde(model, zs, ctx, N, num_steps, cfg_scale, sde)
+        return x[:P * N].reshape(P, N, *shape), dict(nfe=[plan["forwards"]] * P, batch_nfe=plan["forwards"])
     grid = torch.linspace(0, 1, num_steps)            # sample_ode's grid: dopri5 integrates to its last point
     fn = lambda t, x: model.forward_with_cfg(x, t, ctx, cfg_scale)
     y, stats = odeint_dopri5_grouped(fn, torch.cat([zs, zs], 0), flow_batch_row_groups(P, N), P,
@@ -453,7 +528,7 @@ def sample_flow_batched(model, c: dict, uc: dict, num_samples: int, seed: int = 
 
 @torch.no_grad()
 def _conds_to_3d(conditioner, model, decoder, cond_key, prompts, cameras, num_samples, seed, num_steps, cfg_scale,
-                 resolution, dtype):
+                 resolution, dtype, sde):
     """`_cond_to_3d` for a list of conditions: the conditioner once per condition, in order, one batched sample,
     then decode and render of every latent.  The render noise is one device draw for the batch."""
     dev = next(model.parameters()).device
@@ -461,7 +536,7 @@ def _conds_to_3d(conditioner, model, decoder, cond_key, prompts, cameras, num_sa
     c = {k: torch.cat([ci[k] for ci in cs]) if isinstance(cs[0][k], torch.Tensor) else cs[0][k] for k in cs[0]}
     uc = {k: torch.cat([ui[k] for ui in ucs]) if isinstance(ucs[0][k], torch.Tensor) else ucs[0][k] for k in ucs[0]}
     latents, stats = sample_flow_batched(model, c, uc, num_samples, seed=seed, num_steps=num_steps,
-                                         cfg_scale=cfg_scale, dtype=dtype)
+                                         cfg_scale=cfg_scale, dtype=dtype, sde=sde)
     P, N = latents.shape[:2]
     out = decode_and_render(decoder, latents.reshape(P * N, *latents.shape[2:]), cameras[:24].to(dev), resolution)
     return latents, {k: v.reshape(P, N, *v.shape[1:]) for k, v in out.items()}, stats
@@ -470,47 +545,47 @@ def _conds_to_3d(conditioner, model, decoder, cond_key, prompts, cameras, num_sa
 @torch.no_grad()
 def images_to_3d(conditioner, model, decoder, images: torch.Tensor, cameras: torch.Tensor, num_samples: int = 4,
                  seed: int = 42, num_steps: int = 250, cfg_scale: float = 4.0, resolution: int = 192,
-                 dtype=torch.float32):
+                 dtype=torch.float32, sde: dict | None = None):
     """`image_to_3d` with dopri5 for P images (P, 3, H, W) in [-1, 1] in one denoiser batch.  Each image's latents
     are those `image_to_3d` gives for it alone up to the rounding of the batched GEMMs; the renders use one device
-    noise draw for the whole batch, so they are not bit-identical to sequential calls.
+    noise draw for the whole batch, so they are not bit-identical to sequential calls.  `sde`: see sample_flow_batched.
     Returns (latents (P, N, 12, 32, 32), render dict with (P, N, 24, ...) tensors, per-image stats)."""
     dev = next(model.parameters()).device
     imgs = [images[i:i + 1].to(dev).to(dtype).clone() for i in range(images.shape[0])]   # own, aligned buffers
     return _conds_to_3d(conditioner, model, decoder, "img", imgs, cameras, num_samples, seed, num_steps, cfg_scale,
-                        resolution, dtype)
+                        resolution, dtype, sde)
 
 
 @torch.no_grad()
 def mvs_to_3d(conditioner, model, decoder, mv_images: torch.Tensor, mv_cameras: torch.Tensor, cameras: torch.Tensor,
               num_samples: int = 4, seed: int = 42, num_steps: int = 250, cfg_scale: float = 4.0,
-              resolution: int = 192, dtype=torch.float32):
+              resolution: int = 192, dtype=torch.float32, sde: dict | None = None):
     """`mv_to_3d` with dopri5 for P multi-view conditions, mv_images (P, V, 3, H, W) and mv_cameras (P, V, 25), in one
     denoiser batch.  The conditioner runs once per condition in order, so its `aug_c` camera draws follow the same
     sequence as P sequential `mv_to_3d` calls.  Every condition gets its own copy of its views and cameras (the
     conditioner's kernels want 16-byte aligned rows), so with `aug_c=True` the rotations apply to those copies and the
-    caller's `mv_cameras` is left as it is.  Returns as `images_to_3d`."""
+    caller's `mv_cameras` is left as it is.  `sde`: see sample_flow_batched.  Returns as `images_to_3d`."""
     dev = next(model.parameters()).device
     own = lambda x, i: x[i:i + 1].to(dev).to(dtype).clone()
     prompts = [{"img": own(mv_images, i), "c": own(mv_cameras, i)} for i in range(mv_images.shape[0])]
     return _conds_to_3d(conditioner, model, decoder, "img-c", prompts, cameras, num_samples, seed, num_steps,
-                        cfg_scale, resolution, dtype)
+                        cfg_scale, resolution, dtype, sde)
 
 
 @torch.no_grad()
 def _cond_to_3d(conditioner, model, decoder, cond_key, prompt, cameras, num_samples, seed, num_steps, cfg_scale,
-                sampling_method, resolution, dtype):
+                sampling_method, resolution, dtype, sde):
     dev = next(model.parameters()).device
     c, uc = condition_prompt(conditioner, cond_key, prompt, num_samples, device=dev)
     latents = sample_flow(model, c, uc, num_samples, seed=seed, num_steps=num_steps, cfg_scale=cfg_scale,
-                          sampling_method=sampling_method, dtype=dtype)
+                          sampling_method=sampling_method, dtype=dtype, sde=sde)
     return latents, decode_and_render(decoder, latents, cameras[:24].to(dev), resolution)
 
 
 @torch.no_grad()
 def mv_to_3d(conditioner, model, decoder, mv_images: torch.Tensor, mv_cameras: torch.Tensor, cameras: torch.Tensor,
              num_samples: int = 4, seed: int = 42, num_steps: int = 250, cfg_scale: float = 4.0,
-             sampling_method: str = "dopri5", resolution: int = 192, dtype=torch.float32):
+             sampling_method: str = "dopri5", resolution: int = 192, dtype=torch.float32, sde: dict | None = None):
     """Multi-view-to-3D, `FlowMatchingEngine.eval_cldm` for cond_key 'img-c' (nsr/lsgm/flow_matching_trainer.py:
     553-678): the conditioner on {'img': mv_images (1, V, 3, H, W) in [-1, 1], 'c': mv_cameras (1, V, 25)} with the
     unconditional half forced to zero and every row repeated `num_samples` times, `sample_flow`, then decode and render
@@ -519,22 +594,24 @@ def mv_to_3d(conditioner, model, decoder, mv_images: torch.Tensor, mv_cameras: t
 
     The engine casts the views and cameras to its dtype (bf16 under use_amp) before the conditioner sees them; they
     are cast to `dtype` here.  With `aug_c=True` the conditioner rotates cameras of that tensor in place -- the caller's
-    own `mv_cameras` when it already has that dtype and device.  Returns (latents, render dict)."""
+    own `mv_cameras` when it already has that dtype and device.  `sde`: see sample_flow.  Returns (latents, render
+    dict)."""
     dev = next(model.parameters()).device
     img_c = {"img": mv_images.to(dev).to(dtype), "c": mv_cameras.to(dev).to(dtype)}
     return _cond_to_3d(conditioner, model, decoder, "img-c", img_c, cameras, num_samples, seed, num_steps, cfg_scale,
-                       sampling_method, resolution, dtype)
+                       sampling_method, resolution, dtype, sde)
 
 
 @torch.no_grad()
 def image_to_3d(conditioner, model, decoder, image: torch.Tensor, cameras: torch.Tensor, num_samples: int = 4,
                 seed: int = 42, num_steps: int = 250, cfg_scale: float = 4.0, sampling_method: str = "dopri5",
-                resolution: int = 192, dtype=torch.float32):
+                resolution: int = 192, dtype=torch.float32, sde: dict | None = None):
     """Image-to-3D, `FlowMatchingEngine.eval_cldm` for cond_key 'img' (the I23D release): the conditioner on one image
-    (1, 3, H, W) in [-1, 1], `sample_flow`, decode and render of `cameras[:24]`.  Returns (latents, render dict)."""
+    (1, 3, H, W) in [-1, 1], `sample_flow`, decode and render of `cameras[:24]`.  `sde`: see sample_flow.
+    Returns (latents, render dict)."""
     dev = next(model.parameters()).device
     return _cond_to_3d(conditioner, model, decoder, "img", image.to(dev).to(dtype), cameras, num_samples, seed,
-                       num_steps, cfg_scale, sampling_method, resolution, dtype)
+                       num_steps, cfg_scale, sampling_method, resolution, dtype, sde)
 
 
 @torch.no_grad()

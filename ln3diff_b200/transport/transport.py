@@ -1,5 +1,6 @@
 import enum
 
+import numpy as np
 import torch as th
 
 from .. import ops
@@ -41,9 +42,11 @@ class Transport:
 
     def check_interval(self, train_eps, sample_eps, *, diffusion_form="SBDM", sde=False, reverse=False,
                        eval=False, last_step_size=0.0):
-        t0, t1 = 0, 1  # velocity & Linear: stable everywhere (transport.py:85-112)
-        if sde:
-            raise NotImplementedError("SDE sampling is outside the hot path")
+        t0, t1 = 0, 1  # velocity & Linear ODE: stable everywhere (transport.py:85-112)
+        if sde:          # the first step is semi-implicit: SBDM starts at eps, and t1 leaves room for the last step
+            eps = train_eps if not eval else sample_eps
+            t0 = eps if diffusion_form == "SBDM" else 0
+            t1 = 1 - eps if last_step_size == 0 else 1 - last_step_size
         return (1 - t0, 1 - t1) if reverse else (t0, t1)
 
     def get_drift(self):
@@ -52,6 +55,10 @@ class Transport:
             assert out.shape == x.shape, "Output shape from ODE solver must match input shape"
             return out
         return velocity_ode
+
+    def get_score(self):
+        """reference transport.py:231-245 for velocity prediction: path.py get_score_from_velocity."""
+        return lambda x, t, model, **kw: score_from_velocity(model(x, t, **kw), x, t)
 
 
 def create_transport(path_type="Linear", prediction="velocity", loss_weight=None, train_eps=None,
@@ -156,3 +163,274 @@ class Sampler:
                                                eval=True, reverse=reverse, last_step_size=0.0)
         return ode(drift=drift, t0=t0, t1=t1, sampler_type=sampling_method, num_steps=num_steps, atol=atol,
                    rtol=rtol).sample
+
+    def sample_sde(self, *, sampling_method="Euler", diffusion_form="SBDM", diffusion_norm=1.0, last_step="Mean",
+                   last_step_size=0.04, num_steps=250):
+        """reference transport.py:313-372: returns `_sample(init, model, **model_kwargs)`, the list of `num_steps`
+        states of the Euler-Maruyama or Heun SDE solver, the last one from `last_step`.  Every noise draw is the
+        reference's `randn(x.size())` on the global CPU generator.
+
+        With `init` CUDA fp32 and `model` a library denoiser's bound `forward_with_cfg`, each drift evaluation is one
+        forward of the 2N-row CFG batch (a replay of the denoiser's CUDA graph) and one ln3_flow_sde_step; the
+        reference runs the model twice per SDE drift.  Any other model runs the reference's torch arithmetic.
+
+        Raises what the reference raises for an unknown method, diffusion form or last step, NotImplementedError for
+        the `constant` form (the reference cannot run it either: it takes the square root of a Python float), and
+        ValueError where the reference returns NaN: `SBDM` (its diffusion is infinite at t0 = 0 on this transport)
+        and `Heun` with `last_step=None` (its last stage evaluates the score at t = 1, where the variance is 0)."""
+        if last_step is None:
+            last_step_size = 0.0
+        plan = sde_plan(sampling_method, diffusion_form, diffusion_norm, last_step, last_step_size, num_steps,
+                        self.transport)
+        _sde = sde(plan, self.transport)
+
+        def _sample(init, model, **model_kwargs):
+            if init.is_cuda and init.dtype == th.float32 and _is_library_cfg(model):
+                xs = []
+                sde_fused(plan, model.__self__, init, model_kwargs["context"], model_kwargs["cfg_scale"],
+                          lambda k: th.randn(init.size()).to(init), record=xs.append)
+            else:
+                xs = _sde.sample(init, model, **model_kwargs)
+                ts = th.ones(init.size(0), device=init.device) * plan["t1"]
+                xs.append(_sde.last_step(xs[-1], ts, model, **model_kwargs))
+            assert len(xs) == num_steps, "Samples does not match the number of steps"
+            return xs
+        return _sample
+
+
+# ---------------------------------------------------------------------------------------------- SDE sampling
+# The Linear path (alpha_t = t, sigma_t = 1 - t) with velocity prediction: reference path.py:18-110,
+# integrators.py:9-75, transport.py:260-372.
+DIFFUSION_FORMS = ("constant", "SBDM", "sigma", "linear", "decreasing", "inccreasing-decreasing")  # sic, path.py:56
+SDE_METHODS = ("Euler", "Heun")
+LAST_STEPS = (None, "Mean", "Tweedie", "Euler")
+
+
+def _expand(t, x):
+    return t.view(t.size(0), *([1] * (x.dim() - 1)))
+
+
+def score_from_velocity(v, x, t):
+    """path.py:67-82 (ICPlan): (t v - x) / var, var = sigma_t^2 - t * d_sigma_t * sigma_t, in the reference's order."""
+    t = _expand(t, x)
+    sigma_t = 1 - t
+    var = sigma_t ** 2 - t * -1 * sigma_t
+    return (t * v - x) / var
+
+
+def diffusion_coefficient(t, form, norm):
+    """path.py:45-65 (ICPlan.compute_diffusion) for one form; `t` is a float32 tensor."""
+    if form not in DIFFUSION_FORMS:
+        raise NotImplementedError(f"Diffusion form {form} not implemented")
+    if form == "constant":
+        raise NotImplementedError("diffusion_form='constant' is not supported: the reference returns a Python float "
+                                  "there and its th.sqrt(2 * diffusion) raises TypeError")
+    if form == "SBDM":
+        sigma_t = 1 - t
+        return norm * ((1 / t) * (sigma_t ** 2) - sigma_t * -1)
+    if form in ("sigma", "linear"):
+        return norm * (1 - t)
+    if form == "decreasing":
+        return 0.25 * (norm * th.cos(np.pi * t) + 1) ** 2
+    return norm * th.sin(np.pi * t) ** 2
+
+
+class sde:
+    """reference integrators.py:9-75 and transport.py:260-311 in torch arithmetic (two model calls per SDE drift)."""
+
+    def __init__(self, plan, transport):
+        self.plan, self.t, self.dt = plan, plan["grid"], plan["dt"]
+        form, norm = plan["diffusion_form"], plan["diffusion_norm"]
+        self.diffusion = lambda x, t: diffusion_coefficient(_expand(t, x), form, norm)
+        self.drift = transport.get_drift()
+        self.score = transport.get_score()
+
+    def sde_drift(self, x, t, model, **kw):
+        return self.drift(x, t, model, **kw) + self.diffusion(x, t) * self.score(x, t, model, **kw)
+
+    def _euler(self, x, t, model, **kw):
+        w_cur = th.randn(x.size()).to(x)
+        t = th.ones(x.size(0)).to(x) * t
+        dw = w_cur * th.sqrt(self.dt)
+        drift = self.sde_drift(x, t, model, **kw)
+        diffusion = self.diffusion(x, t)
+        mean_x = x + drift * self.dt
+        return mean_x + th.sqrt(2 * diffusion) * dw
+
+    def _heun(self, x, t, model, **kw):
+        w_cur = th.randn(x.size()).to(x)
+        dw = w_cur * th.sqrt(self.dt)
+        t_cur = th.ones(x.size(0)).to(x) * t
+        diffusion = self.diffusion(x, t_cur)
+        xhat = x + th.sqrt(2 * diffusion) * dw
+        K1 = self.sde_drift(xhat, t_cur, model, **kw)
+        xp = xhat + self.dt * K1
+        K2 = self.sde_drift(xp, t_cur + self.dt, model, **kw)
+        return xhat + 0.5 * self.dt * (K1 + K2)   # the last point is not skipped (integrators.py:49)
+
+    def sample(self, init, model, **kw):
+        step = self._euler if self.plan["sampling_method"] == "Euler" else self._heun
+        x, samples = init, []
+        with th.no_grad():
+            for ti in self.t[:-1]:
+                x = step(x, ti, model, **kw)
+                samples.append(x)
+        return samples
+
+    def last_step(self, x, t, model, **kw):
+        kind, size = self.plan["last_step"], self.plan["last_step_size"]
+        if kind is None:
+            return x
+        if kind == "Mean":
+            return x + self.sde_drift(x, t, model, **kw) * size
+        if kind == "Euler":
+            return x + self.drift(x, t, model, **kw) * size
+        alpha, sigma = t[0], 1 - t[0]                  # Tweedie: x / alpha + sigma^2 / alpha * score
+        return x / alpha + (sigma ** 2) / alpha * self.score(x, t, model, **kw)
+
+
+def sde_plan(sampling_method, diffusion_form, diffusion_norm, last_step, last_step_size, num_steps, transport=None):
+    """The drift evaluations of one `sample_sde` run as ln3_flow_sde_step arguments, computed on the host in the
+    reference's float32 arithmetic.  Every entry: the forward time `t` and the kernel's `var`, `diffusion`, `mode`,
+    output coefficients `cx` / `cy` (a, b, c, h, sigma; None: not written), whether it reads the state `x_in` and the
+    history `hist_in`, writes the history `hist_out`, which step's noise it reads (`noise`, or None) and whether its
+    x_out is one of the returned states (`record`).  `pre_sigma`: Heun's first xhat = init + pre_sigma * w_0, before
+    the first forward.  Euler-Maruyama keeps the state in the forward input; Heun keeps xhat in the state."""
+    from .. import ops
+    if sampling_method not in SDE_METHODS:
+        raise NotImplementedError("Smapler type not implemented.")   # integrators.py:61 (sic)
+    if last_step not in LAST_STEPS:
+        raise NotImplementedError(f"last_step={last_step!r}: expected one of {LAST_STEPS}")
+    if num_steps < 2:
+        raise ValueError("sample_sde needs num_steps >= 2 (its step size is t[1] - t[0])")
+    if last_step is None:
+        last_step_size = 0.0
+    if diffusion_form == "SBDM":
+        raise ValueError("diffusion_form='SBDM' is non-finite on this transport: sample_eps = 0 puts the first step at "
+                         "t = 0, where the SBDM diffusion is infinite; use 'sigma' (the command-line default), "
+                         "'linear', 'decreasing' or 'inccreasing-decreasing'")
+    if sampling_method == "Heun" and last_step is None:
+        raise ValueError("sampling_method='Heun' with last_step=None is non-finite: the grid then ends at t1 = 1 and "
+                         "Heun's last stage evaluates the score where its variance is 0; choose a last step")
+    transport = transport or create_transport(snr_type="lognorm")
+    t0, t1 = transport.check_interval(transport.train_eps, transport.sample_eps, diffusion_form=diffusion_form,
+                                      sde=True, eval=True, reverse=False, last_step_size=last_step_size)
+    grid = th.linspace(t0, t1, num_steps)
+    dt = grid[1] - grid[0]
+    sdt = th.sqrt(dt)
+    half = 0.5 * dt
+
+    def at(t):   # t: float32 0-dim tensor -> (t, var, D) as the kernel takes them
+        tt = t.reshape(1)
+        sigma_t = 1 - tt
+        var = sigma_t ** 2 - tt * -1 * sigma_t
+        return dict(t=float(tt), var=float(var), diffusion=float(diffusion_coefficient(tt, diffusion_form,
+                                                                                      diffusion_norm)))
+
+    def noise_scale(t):   # sqrt(2 D(t)) * sqrt(dt)
+        return float(th.sqrt(2 * diffusion_coefficient(t.reshape(1), diffusion_form, diffusion_norm)) * sdt)
+
+    evals = []
+
+    def ev(t, mode, cx, cy=None, *, x_in=False, hist_in=False, hist_out=False, noise=None, record=False):
+        evals.append(dict(at(t), mode=mode, cx=tuple(float(c) for c in cx),
+                          cy=None if cy is None else tuple(float(c) for c in cy), x_in=x_in, hist_in=hist_in,
+                          hist_out=hist_out, noise=noise, record=record))
+
+    S, D, dtf, hf = num_steps - 1, ops.SDE_DRIFT, float(dt), float(half)
+    for i in range(S):
+        if sampling_method == "Euler":               # x <- x + dt (v + D sc) + sqrt(2D) sqrt(dt) w_i
+            c = (0.0, 1.0, dtf, 0.0, noise_scale(grid[i]))
+            ev(grid[i], D, c, c, noise=i, record=True)
+        else:
+            # stage 1 at xhat: K1 -> hist, xhat -> state, xp = xhat + dt K1 -> next input
+            ev(grid[i], D, (0.0, 1.0, 0.0, 0.0, 0.0), (0.0, 1.0, dtf, 0.0, 0.0), hist_out=True)
+            # stage 2 at xp, t + dt in float32: x = xhat + dt/2 (K1 + K2); the next input is the next step's xhat
+            nxt = i + 1 < S
+            cy = (1.0, 0.0, hf, hf, noise_scale(grid[i + 1]) if nxt else 0.0)
+            ev(grid[i] + dt, D, (1.0, 0.0, hf, hf, 0.0), cy, x_in=True, hist_in=True, noise=i + 1 if nxt else None,
+               record=True)
+    t_last = th.ones(1) * t1
+    size = float(th.ones(1) * last_step_size)
+    if last_step == "Mean":
+        ev(t_last, D, (0.0, 1.0, size, 0.0, 0.0), record=True)
+    elif last_step == "Euler":
+        ev(t_last, ops.SDE_VELOCITY, (0.0, 1.0, size, 0.0, 0.0), record=True)
+    elif last_step == "Tweedie":
+        alpha, sigma = t_last, 1 - t_last
+        ev(t_last, ops.SDE_SCORE, (0.0, 1 / alpha, (sigma ** 2) / alpha, 0.0, 0.0), record=True)
+    return dict(sampling_method=sampling_method, diffusion_form=diffusion_form, diffusion_norm=diffusion_norm,
+                last_step=last_step, last_step_size=last_step_size, num_steps=num_steps, t0=t0, t1=t1, grid=grid,
+                dt=dt, evals=evals, pre_sigma=noise_scale(grid[0]) if sampling_method == "Heun" else None,
+                forwards=len(evals))
+
+
+def _is_library_cfg(model) -> bool:
+    """`model` is a library denoiser's bound forward_with_cfg (the fused path's precondition)."""
+    from ..dit._denoiser import DenoiserMixin
+    owner = getattr(model, "__self__", None)
+    return isinstance(owner, DenoiserMixin) and getattr(model, "__func__", None) is type(owner).forward_with_cfg
+
+
+class CfgForward:
+    """The raw forward of a library denoiser on a fixed 2R-row CFG batch through fixed buffers: write the input into
+    `.x`, call with the (2R,) fp32 time rows, read the output (conditional rows first).  A replay of the denoiser's
+    captured graph, or its eager launch sequence under LN3_CUDA_GRAPH=0."""
+
+    def __init__(self, den, context, rows: int, like: th.Tensor):
+        from ..dit._graph import graphs_enabled
+        if den._prep is None:
+            den.prepare()
+        self.den, self.cx = den, den._context(context)
+        self.g = None
+        if graphs_enabled() and not th.cuda.is_current_stream_capturing():
+            self.g = den._graph(rows, self.cx)
+            if self.g.in_scale is not None:
+                self.g.in_scale.fill_(1.0)
+            self.x = self.g.x
+        else:
+            self.x = th.empty((rows,) + tuple(like.shape[1:]), device=like.device, dtype=th.float32)
+
+    def __call__(self, t_rows: th.Tensor) -> th.Tensor:
+        if self.g is None:
+            return self.den._forward_impl(self.x, t_rows, self.cx)
+        self.g.t.copy_(t_rows)
+        self.g.replay()
+        return self.g.out
+
+
+def sde_fused(plan, den, init, context, cfg_scale, draw, record=None):
+    """Run `plan` (sde_plan) on the CUDA fp32 2R-row CFG state `init` around denoiser `den`: one forward and one
+    ln3_flow_sde_step per entry.  `draw(k)` returns step k's noise, a CUDA fp32 (2N, ...) draw (N divides R), and is
+    called once per step in step order; `record(x)` receives every returned state as a new tensor (and, with
+    last_step=None, the last one again).  Returns the final state buffer (2R rows)."""
+    from .. import ops
+    dev, rows = init.device, init.shape[0]
+    fw = CfgForward(den, context, rows, init)
+    t_rows = th.tensor([e["t"] for e in plan["evals"]], dtype=th.float32)[:, None].repeat(1, rows).to(dev)
+    state = th.empty_like(fw.x)
+    hist = th.empty_like(fw.x) if plan["sampling_method"] == "Heun" else None
+    noise, drawn = None, -1
+    fw.x.copy_(init)
+    if plan["pre_sigma"] is not None:               # Heun's first xhat, before the first forward
+        noise, drawn = draw(0), 0
+        P = rows // noise.shape[0]
+        th.add(init.view(2, P, noise.shape[0] // 2, -1), noise.view(2, 1, noise.shape[0] // 2, -1),
+               alpha=plan["pre_sigma"], out=fw.x.view(2, P, noise.shape[0] // 2, -1))
+    last = None
+    for k, e in enumerate(plan["evals"]):
+        f = fw(t_rows[k])
+        if e["noise"] is not None and e["noise"] > drawn:
+            noise, drawn = draw(e["noise"]), e["noise"]
+        x_out = state if record is None or not e["record"] else th.empty_like(state)
+        ops.flow_sde_step(fw.x, f, cfg_scale=cfg_scale, t=e["t"], var=e["var"], diffusion=e["diffusion"],
+                          mode=e["mode"], x=state if e["x_in"] else None, hist=hist if e["hist_in"] else None,
+                          noise=noise if e["noise"] is not None else None, x_out=x_out, cx=e["cx"],
+                          y_out=fw.x if e["cy"] is not None else None, cy=e["cy"] or (0.0,) * 5,
+                          hist_out=hist if e["hist_out"] else None)
+        if x_out is not state:
+            record(x_out)
+            last = x_out
+    if record is not None and plan["last_step"] is None:
+        record(last)
+    return state
