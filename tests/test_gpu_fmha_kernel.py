@@ -20,16 +20,15 @@ p_j = 2^(s_j c - m) (c = scale log2 e):
         bf16 rounding: half a bf16 ulp at |y| + tol.
 Every output is a view inside a NaN-filled buffer whose bytes outside the view must keep their bits, and every
 case is launched three times with bit-identical results."""
-import math
-
 import pytest
 import torch
+
+from kernel_bounds import fmha_reference as reference
+from kernel_bounds import ulp
 
 pytestmark = pytest.mark.gpu
 
 PAD = 256            # NaN elements before and after every output view (512 B of bf16 keeps 16-byte alignment)
-KT = 128             # keys per block of the kernel (for the count of rescales)
-LOG2E = 1.4426950408889634
 
 
 @pytest.fixture(scope="module")
@@ -38,48 +37,6 @@ def dev():
     from ln3diff_b200 import _lib
     _lib.lib()
     return torch.device("cuda", 0)
-
-
-def ulp(v: torch.Tensor, mant_bits: int) -> torch.Tensor:
-    m, e = torch.frexp(v.abs().to(torch.float64))
-    return torch.where(v == 0, torch.zeros_like(v, dtype=torch.float64),
-                       torch.ldexp(torch.ones_like(m), (e - 1 - mant_bits).to(torch.int32)))
-
-
-def heads(t: torch.Tensor, H: int) -> torch.Tensor:
-    """(B, L, H 64) -> (B, H, L, 64) float64."""
-    return t.to(torch.float64).unflatten(2, (H, 64)).transpose(1, 2)
-
-
-def reference(q, k, v, H, scale, causal):
-    """(y, tol) in float64, both (B, Lq, H 64); k / v already hold both K/V sources."""
-    B, Lq, D = q.shape
-    Lkv = k.shape[1]
-    c = scale * LOG2E
-    n_acc = Lkv + 2 * math.ceil(Lkv / KT)
-    ys, tols = [], []
-    step = max(1, (1 << 24) // (H * Lq * Lkv))
-    for b0 in range(0, B, step):
-        qh, kh, vh = (heads(t[b0:b0 + step], H) for t in (q, k, v))
-        s = (qh @ kh.transpose(-1, -2)) * c                        # log2 units
-        a = qh.abs() @ kh.abs().transpose(-1, -2)
-        if causal:
-            mask = torch.ones(Lq, Lkv, dtype=torch.bool, device=q.device).tril()
-            s = s.masked_fill(~mask, -math.inf)
-        m = s.amax(-1, keepdim=True)
-        p = torch.exp2(s - m)                                     # 0 where masked
-        d = c * 64 * 2.0 ** -23 * a + 2.0 ** -22 * (s.abs() + m.abs())
-        e = math.log(2) * d + 2.0 ** -21
-        e = torch.where(p > 0, e, torch.zeros_like(e))
-        l = p.sum(-1, keepdim=True)
-        y = (p @ vh) / l
-        pv = p @ vh.abs()
-        d_num = (p * (e + 2.0 ** -8 * (1 + e))) @ vh.abs() + n_acc * 2.0 ** -23 * (1 + 2.0 ** -7) * pv
-        d_den = (p * e).sum(-1, keepdim=True) + n_acc * 2.0 ** -23 * (p * (1 + e)).sum(-1, keepdim=True)
-        tol = (d_num + y.abs() * d_den) / (l - d_den) + 2.0 ** -23 * y.abs()
-        ys.append(y.transpose(1, 2).flatten(2))
-        tols.append(tol.transpose(1, 2).flatten(2))
-    return torch.cat(ys), torch.cat(tols)
 
 
 def guarded_out(B, Lq, D, ldo, bs, dev):

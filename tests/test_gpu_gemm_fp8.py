@@ -21,18 +21,19 @@ The largest error / bound ratio of each case is printed: if the hardware accumul
 that is what this file reports, and the bound stays where it is derived.
 Outputs sit in NaN-filled buffers whose bytes outside the view must keep their bits, and three launches must give
 identical bits (no split-K, no atomics)."""
-import math
 import zlib
 
 import pytest
 import torch
 
+from kernel_bounds import FP8, SLOPE, fp8_bf16_bound, fp8_out_check, gelu_ref
+from kernel_bounds import fp8_acc_bound as acc_bound
+from kernel_bounds import fp8_head_norm_ref as head_norm_ref
+from kernel_bounds import fp8_reference as reference
+
 pytestmark = pytest.mark.gpu
 
 PAD = 512
-U_ACC = 2.0 ** -13
-SLOPE = 1.13
-FP8 = torch.float8_e4m3fn
 
 
 @pytest.fixture(scope="module")
@@ -41,12 +42,6 @@ def dev():
     from ln3diff_b200 import _lib
     _lib.lib()
     return torch.device("cuda", 0)
-
-
-def ulp(v: torch.Tensor, mant_bits: int) -> torch.Tensor:
-    m, e = torch.frexp(v.abs().to(torch.float64))
-    return torch.where(v == 0, torch.zeros_like(v, dtype=torch.float64),
-                       torch.ldexp(torch.ones_like(m), (e - 1 - mant_bits).to(torch.int32)))
 
 
 def guarded(rows, cols, ld, dtype, dev):
@@ -88,50 +83,8 @@ def operands(M, N, K, dev, seed, bias=True):
     return a_q, a_s.to(dev), w_q, w_s.to(dev), (b.to(dev) if bias else None)
 
 
-def reference(a_q, a_s, w_q, w_s, b):
-    """(y, T) in float64: y the exact scaled GEMM + bias, T the same GEMM on absolute values."""
-    M, K = a_q.shape
-    A = a_q.to(torch.float64).view(M, K // 128, 128) * a_s.to(torch.float64)[:, :, None]
-    A = A.view(M, K)
-    W = w_q.to(torch.float64)
-    y = (A @ W.T) * w_s.to(torch.float64)
-    T = (A.abs() @ W.abs().T) * w_s.to(torch.float64)
-    if b is not None:
-        y = y + b.to(torch.float64)
-    return y, T
-
-
-def acc_bound(T, K, b):
-    bb = b.to(torch.float64).abs() if b is not None else 0.0
-    return 128 * U_ACC * T + (K // 128 + 2) * 2.0 ** -23 * (T + bb)
-
-
-def gelu_ref(x):
-    return 0.5 * x * (1 + torch.special.erf(x / math.sqrt(2))), 1.1e-5 + 3.2e-5 * x.abs()
-
-
-def head_norm_ref(y, E, w, nsec, sec_cols, eps=1e-5):
-    """Per-head RMSNorm of the first nsec sections in float64 and the propagated bound: a perturbation |d_i| <= E_i
-    of the head moves rms by at most max E, so y_i r w_i moves by |w_i| r (E_i + |y_i| r max E) (first order, with
-    a 1 % margin), plus the kernel's own fp32 evaluation (64 products summed, rsqrt, two products: 80 u |out|)."""
-    out, bound = y.clone(), E.clone()
-    M, N = y.shape
-    w = w.to(torch.float64)
-    for sec in range(nsec):
-        for h0 in range(sec * sec_cols, (sec + 1) * sec_cols, 64):
-            if h0 >= N:
-                break
-            yh, Eh = y[:, h0:h0 + 64], E[:, h0:h0 + 64]
-            r = torch.rsqrt((yh * yh).mean(dim=1, keepdim=True) + eps)
-            wh = w[sec][None, :]
-            out[:, h0:h0 + 64] = yh * r * wh
-            bound[:, h0:h0 + 64] = (1.01 * wh.abs() * r * (Eh + yh.abs() * r * Eh.amax(dim=1, keepdim=True))
-                                    + 80 * 2.0 ** -24 * (yh * r * wh).abs())
-    return out, bound
-
-
 def check_bf16(what, got, ref, E):
-    bound = E + 0.5 * ulp(ref.abs() + E, 7)
+    bound = fp8_bf16_bound(ref, E)
     err = (got.to(torch.float64) - ref).abs()
     ratio = float((err / bound.clamp_min(1e-300)).max())
     bad = ~(err <= bound)
@@ -141,27 +94,10 @@ def check_bf16(what, got, ref, E):
 
 def check_fp8(what, q, s, v, d):
     """q / s the kernel's codes and block scales, v the fp64 epilogue value, d its error bound."""
-    M, N = v.shape
-    vb = v.view(M, N // 128, 128)
-    db = d.view(M, N // 128, 128)
-    amax = vb.abs().amax(dim=2)
-    dmax = db.amax(dim=2)
-    s64 = s.to(torch.float64)
-    serr = (s64 * 448 - amax).abs()
-    sbound = dmax + 2.0 ** -22 * amax
-    assert bool((serr <= sbound).all()), f"{what}: block scales off by up to {float((serr / sbound).max()):.3f} x bound"
-    sk = s64[:, :, None]
-    safe = torch.where(sk > 0, sk, torch.ones_like(sk))
-    t = vb / safe
-    dt = db / safe + 2.0 ** -22 * t.abs()
-    rnd = lambda z: z.clamp(-448, 448).to(torch.float32).to(FP8).to(torch.float64)
-    lo, hi = rnd(t - dt), rnd(t + dt)
-    got = q.reshape(M, N // 128, 128).to(torch.float64)
-    zero_blocks = (sk == 0).expand_as(got)
-    ok = torch.where(zero_blocks, got == 0, (got >= lo) & (got <= hi))
+    sratio, exact, ok, s_ok = fp8_out_check(q, s, v, d)
+    assert bool(s_ok.all()), f"{what}: block scales off by up to {sratio:.3f} x bound"
     assert bool(ok.all()), f"{what}: {int((~ok).sum())} of {q.numel()} codes off the restated quantisation"
-    exact = float((got == rnd(t)).to(torch.float64).mean())
-    return float((serr / sbound.clamp_min(1e-300)).max()), exact
+    return sratio, exact
 
 
 CASES = [

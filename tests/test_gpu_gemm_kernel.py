@@ -16,10 +16,11 @@ import tempfile
 import pytest
 import torch
 
+from kernel_bounds import SLOPE, act_ref, gemm_bf16_bound, gemm_tau, head_rmsnorm_ref, ulp
+
 pytestmark = pytest.mark.gpu
 
 PAD = 256           # NaN elements before and after every guarded view (512 B of bf16 keeps 16-byte alignment)
-SLOPE = 1.13        # max |f'| of every activation (GELU 1.129, SiLU / QuickGELU 1.0998 in their scaled argument)
 
 
 @pytest.fixture(scope="module")
@@ -28,12 +29,6 @@ def dev():
     from ln3diff_b200 import _lib
     _lib.lib()
     return torch.device("cuda", 0)
-
-
-def ulp(v: torch.Tensor, mant_bits: int) -> torch.Tensor:
-    m, e = torch.frexp(v.abs().to(torch.float64))
-    return torch.where(v == 0, torch.zeros_like(v, dtype=torch.float64),
-                       torch.ldexp(torch.ones_like(m), (e - 1 - mant_bits).to(torch.int32)))
 
 
 def guarded(shape, ld, dtype, dev, values=None):
@@ -65,31 +60,6 @@ def assert_within(what, got, ref, bound):
                              f"bound {bound.flatten()[i].item():.3e}")
 
 
-# ------------------------------------------------------------------ activations: float64 value and fp32 error
-def act_ref(act, x):
-    """(f(x) in float64, the bound on the kernel's own fp32 evaluation error at x)."""
-    from ln3diff_b200 import ops
-    u = 2.0 ** -24
-    ax = x.abs()
-    if act == ops.ACT_NONE:
-        return x, torch.zeros_like(x)
-    if act == ops.ACT_GELU_ERF:
-        # the default packed polynomial: |abs error| <= 1.1e-5 for |x| < 4 (fp32 evaluation included); beyond,
-        # Phi saturates where the true Phi(4) = 1 - 3.2e-5, so the error is <= 3.2e-5 |x| (and the flushed
-        # negative tail is smaller than |x| Phi(-4) <= 3.2e-5 |x|)
-        return 0.5 * x * (1 + torch.special.erf(x / math.sqrt(2))), 1.1e-5 + 3.2e-5 * ax
-    if act == ops.ACT_GELU_TANH:
-        # 0.5 x (1 + tanhf(arg)): tanhf 2 ulp of |t| <= 1 (2^-22); ~5 roundings in arg move t by
-        # <= 5 u |arg| sech^2(arg) <= 5 u 0.45; the last two products round once each: <= 0.5|x| 2^-21 + 2u|x|
-        k0, k1 = math.sqrt(2 / math.pi), 0.044715
-        return 0.5 * x * (1 + torch.tanh(k0 * (x + k1 * x ** 3))), ax * 2.0 ** -20
-    # x / (1 + __expf(-k x)): __expf is within (2 + 1.173 k|x|) ulp, the rounded argument adds k|x| u relative;
-    # x e / (1 + e)^2 <= |x| / 4 turns e's relative error into the result's; the add and IEEE divide: 2u |x|
-    k = 1.0 if act == ops.ACT_SILU else 1.702
-    rel_e = 2 * u * (2 + 1.173 * k * ax) + k * ax * u
-    return x * torch.sigmoid(k * x), 0.25 * ax * rel_e + 2 * u * ax
-
-
 # ------------------------------------------------------------------ one case
 def run_case(dev, M, N, K, *, bias=True, act=0, out_kind=0, ldo=None, gate_rows=0, out2=False, head_norm=False,
              seed=0):
@@ -101,17 +71,18 @@ def run_case(dev, M, N, K, *, bias=True, act=0, out_kind=0, ldo=None, gate_rows=
     ldo = N if ldo is None else ldo
     a64, w64 = a.double(), w.double()
     y = a64 @ w64.T
-    tau = (a64.abs() @ w64.abs().T)
     if b is not None:
         y = y + b.double()
-        tau = tau + b.double().abs()
-    tau = (K + 1) * 2.0 ** -23 * tau
+    tau = gemm_tau(a64, w64, b.double() if b is not None else None)
 
     kw = {}
     if head_norm:
-        nsec = N // 64
+        # (nsec, sec_cols): every 64-column head its own section, or the production layouts -- sections of D columns
+        # with heads of 64, and columns past the last section left without the norm
+        nsec, sec_cols = (N // 64, 64) if head_norm is True else head_norm
         hw = 1 + 0.1 * torch.randn(nsec, 64, device=dev, generator=g)
-        kw.update(head_norm=hw, head_norm_sec_cols=64, head_norm_eps=1e-6)
+        hn_eps = 1e-6 if head_norm is True else 1e-5
+        kw.update(head_norm=hw, head_norm_sec_cols=sec_cols, head_norm_eps=hn_eps)
     if out_kind == ops.OUT_RESID_F32:
         x0 = torch.randn(M, N, device=dev, generator=g)
         flat, view = guarded((M, N), ldo, torch.float32, dev, x0)
@@ -143,18 +114,8 @@ def run_case(dev, M, N, K, *, bias=True, act=0, out_kind=0, ldo=None, gate_rows=
     got = results[0][0]
 
     if head_norm:
-        # y_n = y rstd w: rstd from the fp32 sum of 64 squares (2 tau / |y| relative per term, 64 u for the sum),
-        # rsqrtf 2 ulp, then two rounded products per element
-        yh = y.view(M, N // 64, 64)
-        th = tau.view(M, N // 64, 64)
-        ms = (yh * yh).mean(-1, keepdim=True)
-        r = torch.rsqrt(ms + 1e-6)
-        rel_r = 0.5 * ((2 * yh.abs() * th + th * th).sum(-1, keepdim=True) / (64 * ms + 64e-6) + 66 * 2.0 ** -24) \
-            + 2.0 ** -22
-        hw64 = hw.double().view(1, N // 64, 64)
-        ref = (yh * r * hw64).reshape(M, N)
-        tol = ((th * r + yh.abs() * r * rel_r) * hw64.abs()).reshape(M, N) + 4 * 2.0 ** -24 * ref.abs()
-        assert_within(what, got, ref, ulp(ref.abs() + tol, 7) / 2 + tol)
+        ref, tol = head_rmsnorm_ref(y, tau, hw, sec_cols, hn_eps)
+        assert_within(what, got, ref, gemm_bf16_bound(ref, tol))
         return
     ref, act_err = act_ref(act, y)
     tol = SLOPE * tau + act_err if act else tau
@@ -229,6 +190,14 @@ def test_residual_output_with_activation(dev):
 
 def test_head_rmsnorm(dev):
     run_case(dev, 333, 1024, 512, bias=True, head_norm=True)
+
+
+@pytest.mark.parametrize("N,nsec", [(3 * 768, 2), (2 * 768, 1)], ids=["qkv-nsec2-D768", "kv-nsec1-D768"])
+def test_head_rmsnorm_sections(dev, N, nsec):
+    """The denoisers' layouts: sections of D = 768 columns with heads of 64 -- qkv of the PixArt blocks (q and k
+    normed, v untouched) and a cross-attention / second-source K|V (K normed, V untouched).  The columns past the
+    last section take the epilogue's `sec >= nsec` skip and must come out as the plain GEMM."""
+    run_case(dev, 333, N, 768, bias=True, head_norm=(nsec, 768))
 
 
 @pytest.mark.parametrize("ldo", [1024 + 64, 512 + 2])

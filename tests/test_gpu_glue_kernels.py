@@ -7,18 +7,20 @@ the view must keep their bits, and an input read outside its view turns the resu
 recomputes its reference with one index mapping deliberately wrong (the neighbouring sample's gate or modulation
 row, resid_rows shifted by one sample, p and q swapped, pos_embed off by one token, the neighbouring plane) and
 asserts that the slip moves the affected elements by >= 100x the tolerance: the data can tell them apart."""
-import math
 import zlib
 
 import numpy as np
 import pytest
 import torch
 
-from oracle import dit as odit
+from kernel_bounds import assert_sensitive, bf16_bound, nm_out_ref, nm_resid_ref, timestep_embedding_ref, ulp_bf16, \
+    ulp_f32
+from kernel_bounds import f32 as _f32
+from kernel_bounds import final_layer_ref as _final_layer_ref
+from kernel_bounds import patch_embed_ref as _patch_ref
 
 pytestmark = pytest.mark.gpu
 
-U32 = 2.0 ** -24      # unit roundoff of fp32
 NAN_PAD = 64          # elements of NaN before and after every guarded view: 256 B of fp32 keeps 32-byte alignment
 
 
@@ -31,26 +33,6 @@ def dev():
 
 
 # ------------------------------------------------------------------ helpers
-def _f32(t: torch.Tensor) -> torch.Tensor:
-    """Round a float64 tensor to fp32 (one IEEE round-to-nearest) and keep it in float64."""
-    return t.to(torch.float32).to(torch.float64)
-
-
-def _ulp(v: torch.Tensor, mant_bits: int) -> torch.Tensor:
-    """Spacing of the floating-point grid with `mant_bits` stored mantissa bits at |v| (0 at v == 0)."""
-    m, e = torch.frexp(v.to(torch.float64))
-    u = torch.ldexp(torch.ones_like(m), (e - 1 - mant_bits).to(torch.int32))
-    return torch.where(v == 0, torch.zeros_like(u), u)
-
-
-def ulp_f32(v):
-    return _ulp(v, 23)
-
-
-def ulp_bf16(v):
-    return _ulp(v, 7)
-
-
 def assert_within(what: str, got: torch.Tensor, ref: torch.Tensor, bound: torch.Tensor) -> None:
     got = got.detach().cpu().to(torch.float64)
     ref, bound = ref.to(torch.float64), bound.to(torch.float64).expand_as(ref)
@@ -62,19 +44,6 @@ def assert_within(what: str, got: torch.Tensor, ref: torch.Tensor, bound: torch.
         idx = tuple(int(i) for i in np.unravel_index(int(score.flatten().argmax()), tuple(got.shape)))
         raise AssertionError(f"{what}: {int(bad.sum())} of {got.numel()} elements out of bound; worst at index {idx}: "
                              f"got {got[idx].item()!r} expected {ref[idx].item()!r} bound {bound[idx].item():.3e}")
-
-
-def assert_sensitive(what: str, ref: torch.Tensor, wrong: torch.Tensor, tol: torch.Tensor,
-                     affected: torch.Tensor | None = None) -> None:
-    """The reference with one index mapping wrong must differ from the true one by >= 100x the tolerance on the
-    affected elements (median, so that elements whose operands happen to coincide do not decide it)."""
-    tol = tol.to(torch.float64).expand_as(ref)
-    ratio = (wrong - ref).abs() / tol.clamp_min(1e-300)
-    if affected is not None:
-        ratio = ratio[affected.expand_as(ref)]
-    assert ratio.numel() > 0, f"{what}: the slip affects no element"
-    med = float(ratio.median())
-    assert med >= 100.0, f"{what}: a slip moves the affected elements by only {med:.1f}x the tolerance (median)"
 
 
 class Guarded:
@@ -112,101 +81,7 @@ def _dev64(t: torch.Tensor) -> torch.Tensor:
     return t.detach().cpu().to(torch.float64)
 
 
-# ------------------------------------------------------------------ norm_modulate: reference
-def nm_tau(x: torch.Tensor, norm: int, nhat: torch.Tensor, w, one_p_s1, s0, y: torch.Tensor) -> torch.Tensor:
-    """Error of the fp32 statistics and the modulation roundings of one norm_modulate / final_layer row, before
-    the bf16 rounding.  A lane sums D/32 values, then 5 shuffle levels, then the division: every fp32 sum here has
-    at most k = D/32 + 8 rounded additions, so its relative error is <= gamma = k * 2^-24 (Higham 3.1):
-      LAYER  |mean error| <= gamma * mean|x|; rstd's relative error <= gamma/2 (variance) + 2^-22 (rsqrtf, 2 ulp)
-             + 2^-24 (the eps add);
-      RMS    no mean, the same rstd term;
-      n^ = (x - mean) * rstd: two more roundings; * weight and the fma with (1 + scale): one each (2^-23 * |y|),
-    so tau = |w (1 + s1)| * (rstd * |mean error| + |n^| * (gamma + 2^-21)) + 2^-23 * (|y| + |s0|)."""
-    if norm == 0:
-        return torch.zeros_like(y)
-    D = x.shape[-1]
-    gamma = (D / 32 + 8) * U32
-    if norm == 1:
-        mean_err = gamma * x.abs().mean(-1, keepdim=True)
-        rstd = torch.rsqrt(((x - x.mean(-1, keepdim=True)) ** 2).mean(-1, keepdim=True) + 1e-6)
-    else:
-        mean_err = torch.zeros_like(x[..., :1])
-        rstd = torch.rsqrt((x * x).mean(-1, keepdim=True) + 1e-6)
-    amp = torch.ones_like(y)
-    if w is not None:
-        amp = amp * w.abs()
-    if one_p_s1 is not None:
-        amp = amp * one_p_s1.abs()
-    t = amp * (rstd * mean_err + nhat.abs() * (gamma + 2.0 ** -21)) + 2.0 ** -23 * y.abs()
-    if s0 is not None:
-        t = t + 2.0 ** -23 * s0.abs()
-    return t
-
-
-ACT_REF = {  # act -> (float64 function, tau(x, y)): kernel error before the bf16 rounding
-    # x / (1 + __expf(-x)): __expf is within (2 + 1.173|x|) ulp, the add and the IEEE divide round once each
-    3: (lambda v: v * torch.sigmoid(v), lambda v, y: y.abs() * (3 + 1.2 * v.abs()) * 2.0 ** -23),
-    # 0.5 x (1 + erff(x / sqrt2)): erff 2 ulp of |erf| <= 1, the scaled argument moves erf by <= 2^-24,
-    # three more roundings on the product: 0.5 |x| * 2^-21 + 2^-22 |y|
-    1: (lambda v: 0.5 * v * (1 + torch.erf(v / math.sqrt(2))), lambda v, y: 2.0 ** -22 * (v.abs() + y.abs())),
-    # 0.5 x (1 + tanhf(k0 (x + k1 x^3))): the argument carries 5 roundings (relative 5 * 2^-24, tanh' <= 1),
-    # tanhf 2 ulp; then 1 +, 0.5 x *: 0.5 |x| (5 * 2^-24 |arg| + 2^-22) + 2^-22 |y|
-    2: (lambda v: 0.5 * v * (1 + torch.tanh(math.sqrt(2 / math.pi) * (v + 0.044715 * v ** 3))),
-        lambda v, y: 0.5 * v.abs() * (5 * U32 * (0.8 * v.abs() + 0.036 * v.abs() ** 3) + 2.0 ** -22)
-        + 2.0 ** -22 * y.abs()),
-}
-
-
-def nm_resid_ref(x, resid, gate, gate_idx, bcast=None, bcast_idx=None, inside=None, ogate=None, ogate_idx=None):
-    """The kernel's residual update, one fp32 fmaf(g, r, x) per term: g * r (fp32 x bf16) is exact in float64, so
-    rounding the float64 sum to fp32 matches fmaf except where a tie of the double rounding lands (<= 1 ulp).
-    Outside rows with resid_out_gate add their own gated row first, then the ungated broadcast row."""
-    if resid is None:
-        return x.clone()
-    rows = x.shape[0]
-    g = gate[gate_idx] if gate is not None else torch.ones_like(x)
-    if bcast is None:
-        return _f32(x + g * resid)
-    out = torch.empty_like(x)
-    ins = inside if inside is not None else torch.ones(rows, dtype=torch.bool)
-    out[ins] = _f32(x[ins] + g[ins] * resid[ins])
-    o = ~ins
-    if ogate is not None:
-        t = _f32(x[o] + ogate[ogate_idx[o]] * resid[o])
-        out[o] = _f32(t + bcast[bcast_idx[o]])
-    else:
-        out[o] = _f32(x[o] + g[o] * bcast[bcast_idx[o]])
-    return out
-
-
-def nm_out_ref(xn, norm, eps, act, weight=None, shift=None, scale=None, mod_idx=None, shift_tab=None, scale_tab=None):
-    """bf16 output before its rounding, from the (updated) fp32 row xn; returns (y, tau)."""
-    if norm == 1:
-        nhat = odit.layer_norm(xn, eps)
-    elif norm == 2:
-        nhat = odit.rms_norm(xn, None, eps)
-    else:
-        nhat = xn
-    y = nhat * weight if weight is not None else nhat
-    one_p, s0 = None, None
-    if shift is not None:
-        s1, s0 = scale[mod_idx], shift[mod_idx]
-        if scale_tab is not None:
-            s1, s0 = _f32(s1 + scale_tab), _f32(s0 + shift_tab)   # the kernel adds the tables in fp32
-        one_p = _f32(1 + s1)                                    # and rounds 1 + scale before the fma
-        y = y * one_p + s0
-    tau = nm_tau(xn, norm, nhat, weight, one_p, s0, y)
-    if act:
-        f, tau_act = ACT_REF[act]
-        y, tau = f(xn), tau_act(xn, f(xn))                      # activations run with LN3_NORM_NONE only
-    return y, tau
-
-
-def bf16_bound(y, tau):
-    """bf16 output = the fp32 value rounded once: half a bf16 ulp of the exact value plus the fp32 error tau."""
-    return ulp_bf16(y) / 2 + tau
-
-
+# ------------------------------------------------------------------ norm_modulate: reference (kernel_bounds.py)
 def check_x(what, got, ref):
     """fp32 residual stream: at most 1 ulp (double-rounding ties only), and bit-exact almost everywhere."""
     assert_within(what, got, ref, ulp_f32(ref))
@@ -439,26 +314,6 @@ def test_norm_modulate_split_pass_row_slice(dev, D, g0, g1):
 
 
 # ------------------------------------------------------------------ final_layer
-def _final_layer_ref(x, shift, scale, W, bias, S, Cout, shift_tab=None, scale_tab=None, swap_pq=False):
-    """(out, bound) in float64: LN (eps 1e-6) -> modulate with the kernel's fp32 roundings -> Linear -> unpatchify."""
-    B = x.shape[0]
-    s1, s0 = scale[:, None, :], shift[:, None, :]
-    if scale_tab is not None:
-        s1, s0 = _f32(s1 + scale_tab), _f32(s0 + shift_tab)
-    one_p = _f32(1 + s1)
-    nhat = odit.layer_norm(x, 1e-6)
-    y = nhat * one_p + s0
-    tau = nm_tau(x, 1, nhat, None, one_p, s0, y)
-    feat = y @ W.t() + (bias if bias is not None else 0)
-    # fp32 dot product of D terms plus the bias: (n_terms + 4) * 2^-24 * sum|terms|, plus the LN error carried
-    # through the weights, sum_d |W_od| * tau_d
-    terms = y.abs() @ W.abs().t() + (bias.abs() if bias is not None else 0)
-    fb = (x.shape[-1] + 1 + 4) * U32 * terms + tau @ W.abs().t()
-    if swap_pq:      # feature index (p * 2 + q) * Cout + c read with p and q exchanged
-        feat = feat.reshape(B, -1, 2, 2, Cout).transpose(2, 3).reshape(feat.shape)
-    return odit.unpatchify_rollout(feat, Cout), odit.unpatchify_rollout(fb, Cout)
-
-
 FL_CASES = {  # id: (D, Cout, S, B, tables, bias)
     "pair-768-S32-B2": (768, 4, 32, 2, False, True),
     "pair-768-S32-B1": (768, 4, 32, 1, False, True),
@@ -534,24 +389,6 @@ def test_final_layer_rejects_unpaired_or_malformed_tables(dev):
 
 
 # ------------------------------------------------------------------ patch_embed
-def _patch_ref(x, in_scale, W, bias, pos, roll_pos=False, roll_plane=False, roll_scale=False):
-    """(tokens, bound) in float64.  The kernel scales x in fp32 (one rounding), then acc = bias, one fmaf per
-    input, + pos_embed: (n_terms + 4) * 2^-24 * sum|terms| with n_terms = 4 Cin + 2."""
-    B, C3, S, _ = x.shape
-    if in_scale is not None:
-        s = in_scale.roll(1, 0) if roll_scale else in_scale
-        x = _f32(s[:, None, None, None] * x)
-    if roll_plane:   # the patch of the neighbouring plane n
-        x = x.reshape(B, C3 // 3, 3, S, S).roll(1, 2).reshape(x.shape)
-    tok = odit.patch_embed_rollout({"x_embedder.proj.weight": W, "x_embedder.proj.bias": bias}, x)
-    terms = odit.patch_embed_rollout({"x_embedder.proj.weight": W.abs(),
-                                      "x_embedder.proj.bias": bias.abs() if bias is not None else None}, x.abs())
-    if pos is not None:
-        p = pos.roll(1, 0) if roll_pos else pos
-        tok, terms = tok + p, terms + pos.abs()
-    return tok, (4 * C3 // 3 + 2 + 4) * U32 * terms
-
-
 PE_CASES = {  # id: (Cin, D, S, B, in_scale, bias, pos)     Cin = 4 and D % 4 == 0 -> patch_embed_k16_kernel
     "k16-S32-B2": (4, 768, 32, 2, False, True, True),
     "k16-S6-B5-scale": (4, 768, 6, 5, True, True, True),
@@ -621,17 +458,10 @@ def test_timestep_embedding(dev, B):
     ops.timestep_embedding(Guarded(t, dev).view, out=out.view)
     torch.cuda.synchronize()
     out.check("embedding")
-    # the oracle's fp32 frequencies (torch.exp of the fp32 exponent); the argument t * f exactly
-    freqs = torch.exp(-math.log(10000.0) * torch.arange(128, dtype=torch.float32) / 128).double()
-    arg = t.double()[:, None] * freqs[None]
-    ref = torch.cat([arg.cos(), arg.sin()], -1)
-    # the kernel's fp32 argument: expf vs torch.exp (1 ulp each way) and the rounded product t * f, both
-    # relative <= 2^-23 * t f <= 2^-23 |t| (f <= 1); cosf / sinf add 2 ulp of a value <= 1: tau = 2^-22 (|t| + 1)
-    tau = 2.0 ** -22 * (t.double().abs()[:, None] + 1)
-    bound = ulp_bf16(ref) / 2 + tau
+    ref, bound = timestep_embedding_ref(t)
     assert_within(f"B={B}: [cos | sin]", out.view, ref, bound)
     if B > 1:
-        wrong = torch.cat([(arg.roll(1, 0)).cos(), (arg.roll(1, 0)).sin()], -1)
+        wrong = timestep_embedding_ref(t.roll(1, 0))[0]
         assert_sensitive("neighbouring sample's t", ref, wrong, bound, (t != t.roll(1, 0))[:, None])
     assert_sensitive("cos and sin halves swapped", ref, ref.roll(128, 1), bound)
 

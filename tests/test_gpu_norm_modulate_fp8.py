@@ -11,9 +11,10 @@ code = e4m3_rne_satfinite(fp32(y / s)); an all-zero block has s = 0 and zero cod
 import pytest
 import torch
 
-pytestmark = pytest.mark.gpu
+from kernel_bounds import nm_fp8_error
+from kernel_bounds import restated_fp8 as restated
 
-FP8 = torch.float8_e4m3fn
+pytestmark = pytest.mark.gpu
 
 
 @pytest.fixture(scope="module")
@@ -22,23 +23,6 @@ def dev():
     from ln3diff_b200 import _lib
     _lib.lib()
     return torch.device("cuda", 0)
-
-
-def restated(y32: torch.Tensor):
-    """The format evaluated by torch on fp32 values: (codes, scales)."""
-    rows, D = y32.shape
-    b = y32.view(rows, D // 128, 128)
-    amax = b.abs().amax(dim=2)
-    s = amax / torch.full_like(amax, 448.0)         # a true division: torch turns `/ 448.0` into `* (1/448)`
-    safe = torch.where(s > 0, s, torch.ones_like(s))
-    t = torch.where(s[:, :, None] > 0, b / safe[:, :, None], torch.zeros_like(b))
-    return t.clamp(-448, 448).to(FP8).view(rows, D), s
-
-
-def half_ulp_e4m3(t: torch.Tensor) -> torch.Tensor:
-    """Half the e4m3 spacing at |t| (subnormal spacing 2^-9 below 2^-6)."""
-    _, e = torch.frexp(t.abs().to(torch.float64).clamp_min(2.0 ** -6))
-    return torch.ldexp(torch.full_like(t, 0.5, dtype=torch.float64), (e - 1 - 3).to(torch.int32))
 
 
 def inputs(rows, D, dev, seed):
@@ -96,11 +80,7 @@ def test_norm_modulate_fp8_within_half_ulp(dev, norm_kind, rows, D, T):
     sc, sh = scale.double()[idx], shift.double()[idx]
     y = n * (1 + sc) + sh
     e = 64 * 2.0 ** -24 * (n.abs() * (1 + sc.abs()) + sh.abs())
-    s64 = s.double().repeat_interleave(128, dim=1)
-    deq = q.double() * s64
-    safe = torch.where(s64 > 0, s64, torch.ones_like(s64))
-    bound = half_ulp_e4m3((y.abs() + e) / safe) * s64 + e + 2.0 ** -22 * y.abs()
-    err = (deq - y).abs()
+    err, bound = nm_fp8_error(q, s, y, e)
     assert bool((err <= bound).all()), f"{int((err > bound).sum())} values off; max ratio {float((err / bound).max()):.3f}"
     print(f"{norm_kind} {rows}x{D}: max error / bound {float((err / bound).max()):.3e}")
 
