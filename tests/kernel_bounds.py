@@ -1,6 +1,7 @@
 """TEST INFRASTRUCTURE ONLY -- the float64 references and error bounds of the CUDA kernels, shared by the per-kernel
 tests (test_gpu_gemm_kernel.py, test_gpu_fmha_kernel.py, test_gpu_glue_kernels.py, test_gpu_gemm_fp8.py,
-test_gpu_norm_modulate_fp8.py) and the launch audit of the DiT denoisers (test_gpu_denoiser_launches.py).  Each
+test_gpu_norm_modulate_fp8.py, test_gpu_decoder_conv_conformance.py, test_gpu_vae_encoder.py, test_gpu_vae_xl.py)
+and the launch audits of the DiT denoisers and the VAE (test_gpu_denoiser_launches.py, test_gpu_vae_launches.py).  Each
 bound is derived from its kernel's arithmetic in the docstring or comment beside it; the product package never
 imports this module."""
 from __future__ import annotations
@@ -8,6 +9,7 @@ from __future__ import annotations
 import math
 
 import torch
+import torch.nn.functional as F
 
 from oracle import dit as odit
 
@@ -433,3 +435,205 @@ def nm_fp8_error(q, s, y, e):
     safe = torch.where(s64 > 0, s64, torch.ones_like(s64))
     bound = half_ulp_e4m3((y.abs() + e) / safe) * s64 + e + 2.0 ** -22 * y.abs()
     return (deq - y).abs(), bound
+
+
+# ------------------------------------------------------------------ NHWC conv / GroupNorm / single-head attention /
+# tri-plane patch embed (decoder_conv.cu)
+SWISH_SLOPE = 1.1         # max |d/dz z sigmoid(z)| = 1.0998
+KB = 32                   # keys per block of ln3_attn_single_head
+
+
+def _expf_rel(z):
+    """__expf(x) error relative to exp(x): at most 2 + floor(|1.173 x|) ulp (CUDA programming guide), an ulp <= 2u."""
+    return (2 + torch.floor(1.173 * z.abs())) * 2 * U32
+
+
+def _swish_tol(z, dz):
+    """Error of the kernel's v / (1 + __expf(-v)) with v = z + dz (|dz| the error of the fp32 pre-activation):
+    the input error passes with slope <= 1.1; __expf(-v) is off by _expf_rel relative, which moves 1 + e and so the
+    quotient by at most that much relative; the add and the division round once each (2u).  Below z = -88.7
+    __expf(-v) overflows to inf and the kernel returns -0: the whole value |s| is lost there (and is < 3e-37), and the
+    2^-126 floor covers quotients that fall into the subnormal range."""
+    s = z * torch.sigmoid(z)
+    rel = torch.where(z < -80, torch.ones_like(z), _expf_rel(z) + 3 * U32)
+    return s, SWISH_SLOPE * dz + s.abs() * rel + 2.0 ** -126
+
+
+def conv_reference(x, w, b, *, ksize, up, sc=None, sh=None, swish=False, res=None, tf32=False, dz=None):
+    """(ref, tol) in float64, NCHW.  x fp32 NHWC (N, Hin, Win, Cin) on the device; sc, sh fp32 (N, Cin) are the very
+    values the kernel gets, so the reference input is x_hat = swish(x sc + sh) evaluated in float64 and this isolates
+    the conv.  Per output element, with T = conv(|x_hat|, |w|) + |b| and K = ksize^2 Cin:
+      fp32: a chain of K fmaf plus the bias add: (K + 4) u T;
+      TF32: both operands rounded to nearest 10-bit mantissas (2^-11 relative each) before the fp32-accumulated
+            mma: 2^-10 T more;
+      input: the kernel's x_hat is off by d = u |z| (the fmaf z = x sc + sh rounds once), passed through swish by
+            _swish_tol, and the conv carries d through |w|: conv(d, |w|) (times 1 + 2^-9 for the TF32 rounding of
+            the perturbed value);
+      residual: the final add rounds once more, u |out|.
+    dz (N, Hin, Win, Cin) adds an upstream error of z (the composed GroupNorm test)."""
+    x64 = x.double()
+    d = torch.zeros_like(x64)
+    if sc is not None:
+        z = x64 * sc.double()[:, None, None, :] + sh.double()[:, None, None, :]
+        d = U32 * z.abs() + (dz if dz is not None else 0.0)
+        if swish:
+            xh, d = _swish_tol(z, d)
+        else:
+            xh = z
+    else:
+        xh = x64
+    xh, d = xh.permute(0, 3, 1, 2), d.permute(0, 3, 1, 2)
+    if up:
+        xh, d = F.interpolate(xh, scale_factor=2.0, mode="nearest"), F.interpolate(d, scale_factor=2.0, mode="nearest")
+    w64 = w.double()
+    pad = ksize // 2
+    ref = F.conv2d(xh, w64, None if b is None else b.double(), padding=pad)
+    T = F.conv2d(xh.abs(), w64.abs(), None if b is None else b.double().abs(), padding=pad)
+    K = ksize * ksize * x.shape[3]
+    tol = ((2.0 ** -10 if tf32 else 0.0) + (K + 4) * U32) * T + (1 + 2.0 ** -9) * F.conv2d(d, w64.abs(), padding=pad)
+    if res is not None:
+        ref = ref + res.double().permute(0, 3, 1, 2)
+        tol = tol + U32 * ref.abs()
+    return ref, tol
+
+
+def gn_reference(x, gamma, beta, G, eps=1e-6):
+    """(sc, sh, tol_sc, tol_sh, e_mu, mu) in float64, each (N, C).  The kernel, per (image, group) of cnt = HW C/G
+    elements: each of 256 threads adds m = ceil(cnt / 256) terms in sequence, then a 5-level shuffle tree in each warp
+    and a 5-level tree over the 8 warp sums, so every term meets at most m + 10 roundings; the mean divides once more:
+      e_mu  <= (m + 11) u A,   A = sum |x| / cnt.
+    The second pass adds fmaf(d, d, q) of d = fl(x - mu_hat) (2u relative on d^2) over the same m + 10 levels, and
+    sum (x - mu_hat)^2 = sum (x - mu)^2 + cnt e_mu^2, so with var = biased variance
+      |var_hat - var| <= (m + 13) u var + e_mu^2        (the division by cnt included).
+    var + eps rounds (u) and rsqrtf is within 2 ulp (4u), so rstd is off by rel_r = 1/2 rel(var + eps) + 4u; then
+      sc = fl(gamma rstd):               |d sc| <= |sc| (rel_r + u)
+      sh = fl(beta - fl(mu_hat sc_hat)): |d sh| <= |sc| e_mu + |mu| |d sc| + u |mu sc| + u |sh|
+    every term taken 1 % larger for the second-order products."""
+    N, H, W, Cc = x.shape
+    cpg, cnt = Cc // G, H * W * Cc // G
+    m = -(-cnt // 256)
+    xg = x.double().reshape(N, H * W, G, cpg)
+    mu = xg.mean(dim=(1, 3))                                             # (N, G)
+    var = ((xg - mu[:, None, :, None]) ** 2).mean(dim=(1, 3))
+    A = xg.abs().mean(dim=(1, 3))
+    e_mu = 1.01 * (m + 11) * U32 * A
+    e_var = 1.01 * ((m + 13) * U32 * var + e_mu ** 2)
+    rstd = 1 / torch.sqrt(var + eps)
+    rel_r = 1.01 * (0.5 * (e_var / (var + eps) + U32) + 4 * U32)
+    rep = lambda t: t.repeat_interleave(cpg, dim=1)                      # (N, G) -> (N, C)
+    g64, b64 = gamma.double()[None], beta.double()[None]
+    sc = g64 * rep(rstd)
+    sh = b64 - rep(mu) * sc
+    tol_sc = 1.01 * sc.abs() * (rep(rel_r) + U32)
+    tol_sh = 1.01 * (sc.abs() * rep(e_mu) + rep(mu).abs() * tol_sc + U32 * (rep(mu) * sc).abs() + U32 * sh.abs())
+    return sc, sh, tol_sc, tol_sh, rep(e_mu), rep(mu)
+
+
+def attn_reference(q, k, v):
+    """(y, tol) in float64, (N, L, C).  The kernel pre-multiplies q by scale = fl(1 / sqrtf(C)) (scale 2u off the exact
+    C^-1/2, the product one more rounding), scores s_j with a C-term fmaf chain, so with a_j = C^-1/2 sum |q k_j|
+      |d s_j| <= (C + 4) u a_j;
+    p_j = __expf(fl(s_j - m)) with m the running max of the scores: the subtraction rounds (u |s_j - m|) and __expf adds
+    _expf_rel(s_j - m).  Shifting every score by the same m does not change the ratio, so m's own error drops out, and
+    |s_j - m| is largest with the final m, which the reference uses.  When a block raises the running max from m_old to
+    m_new, the kernel multiplies the numerator and the denominator accumulated so far by alpha = __expf(fl(m_old - m_new)).
+    That scales the keys already seen against the later ones, so alpha's own error is charged to each earlier key: key j
+    sees at most nb - 1 such rescales (nb = ceil(L / 32)), each with |m_old - m_new| <= m - s_j + 2 d_max (m_old >= s_j
+    since key j is already in, m_new <= m; d_max = the largest |d s|), so each is off by at most
+      eps_j = expm1(u r_j) + _expf_rel(r_j),  r_j = |s_j - m| + 2 d_max.
+    P stays fp32, so the relative error of the kernel's weight of key j is
+      e_j   = (1 + expm1((C + 4) u a_j + u |s_j - m|) + _expf_rel(s_j - m)) (1 + eps_j)^(nb - 1) - 1
+            (1 below -80, where ex2.approx flushes to 0)
+      num   |d num| <= sum_j p_j |v_j| e_j + n_acc 2u sum_j p_j |v_j| (1 + e_j)
+      den   |d l|   <= sum_j p_j e_j + n_acc 2u sum_j p_j (1 + e_j)
+      n_acc = L + 2 ceil(L / 32): one add per key (the 5-level block sum adds only the block's keys), one rescale
+              product per 32-key block in each accumulator
+      y     (|d num| + |y| |d l|) / (l - |d l|) + 2u |y| (1 / l and the product)."""
+    N, L, Cc = q.shape
+    q64, k64, v64 = q.double(), k.double(), v.double()
+    sc = Cc ** -0.5
+    s = (q64 @ k64.transpose(1, 2)) * sc
+    a = (q64.abs() @ k64.abs().transpose(1, 2)) * sc
+    m = s.amax(-1, keepdim=True)
+    p = torch.exp(s - m)
+    arg = (s - m).abs()
+    nb = math.ceil(L / KB)
+    r = arg + 2 * (Cc + 4) * U32 * a.amax(-1, keepdim=True)
+    eps = torch.expm1(U32 * r) + _expf_rel(r)
+    e = (1 + torch.expm1((Cc + 4) * U32 * a + U32 * arg) + _expf_rel(arg)) * (1 + eps) ** (nb - 1) - 1
+    e = torch.where(arg > 80, torch.ones_like(e), e)
+    n_acc = L + 2 * nb
+    l = p.sum(-1, keepdim=True)
+    y = (p @ v64) / l
+    d_num = (p * e) @ v64.abs() + n_acc * 2 * U32 * ((p * (1 + e)) @ v64.abs())
+    d_den = (p * e).sum(-1, keepdim=True) + n_acc * 2 * U32 * (p * (1 + e)).sum(-1, keepdim=True)
+    tol = (d_num + y.abs() * d_den) / (l - d_den) + 2 * U32 * y.abs()
+    return y, tol
+
+
+def pet_reference(lat, w, b, in_mul):
+    """(tokens, tol_tok, silu, tol_silu) in float64.  The kernel input is fl(lat in_mul), the same rounding torch does
+    for `lat * in_mul`, so the reference starts from that fp32 product.  Each token is a chain of K = 4 Cz fmaf
+    started from the bias: |d tok| <= (4 Cz + 2) u T, T = sum |w x| + |b|.  The bf16 copy is
+    fl_bf16(silu_k(tok_hat)): swish of a value off by d tok (_swish_tol), then round to nearest bf16: half an ulp of
+    8 significant bits, up to 2^-8 |silu| just above a power of two (+ 2^-8 of its error, and half the 2^-133 spacing
+    below bf16's normal range)."""
+    B, C3, S, _ = lat.shape
+    Cz, E = C3 // 3, w.shape[0] // 3
+    x = (lat * in_mul).double()                                       # fp32 product, as torch rounds it
+    w64 = w.double()
+    y = F.conv2d(x, w64, None if b is None else b.double(), stride=2, groups=3)
+    T = F.conv2d(x.abs(), w64.abs(), None if b is None else b.double().abs(), stride=2, groups=3)
+    tok = lambda t: t.reshape(B, E, 3, S // 2, S // 2).flatten(2).transpose(1, 2)     # B (3 h w) E
+    y, T = tok(y), tok(T)
+    tol = (4 * Cz + 2) * U32 * T
+    silu, tol_s = _swish_tol(y, tol)
+    tol_s = tol_s * (1 + 2.0 ** -8) + 2.0 ** -8 * silu.abs() + 2.0 ** -134
+    return y, tol, silu, tol_s
+
+
+# ------------------------------------------------------------------ encoder Downsample, VAE posterior, view mean
+def downsample_reference(x, w, b, tf32):
+    """(ref, tol) in float64, NCHW, of F.conv2d(F.pad(x, (0,1,0,1)), w, b, stride=2); x NHWC fp32, w (Cout, Cin, 3, 3).
+    Per element, with T = sum |w x| + |b| over the K = 9 Cin terms:
+      fp32: a chain of K fused multiply-adds plus the bias add, |err| <= (K + 4) 2^-24 T;
+      TF32: both operands rounded to 10-bit mantissas (relative 2^-11 each, so 2^-10 per product) on top of the
+            fp32 accumulation: |err| <= (2^-10 + (K + 4) 2^-24) T."""
+    xc = x.double().permute(0, 3, 1, 2)
+    w64, b64 = w.double(), b.double()
+    ref = F.conv2d(F.pad(xc, (0, 1, 0, 1)), w64, b64, stride=2)
+    T = F.conv2d(F.pad(xc.abs(), (0, 1, 0, 1)), w64.abs(), stride=2) + b64.abs()[:, None, None]
+    K = 9 * x.shape[3]
+    return ref, ((2.0 ** -10 if tf32 else 0.0) + (K + 4) * U32) * T
+
+
+def _posterior_tol(qw, qb, mom, mean, lv, z, noise):
+    """Float64 vs kernel (an ulp is at most 2^-23 = 2u of the value).  Moments: an 8-term fmaf chain plus the bias add,
+    <= 9u T (T = sum |w h| + |b|, mom NCHW).  logvar: the input error passes tanh with slope <= 1; div (1/2 ulp), tanhf (2 ulp)
+    and mul (1/2 ulp) add 3 ulp <= 6u |lv|, bounded by 8u.  std = exp(0.5 lv): 0.5 lv is exact, so a relative error of
+    0.5 err(lv) + 2 ulp (expf) = 0.5 err(lv) + 4u; the product std * noise adds u, the final sum u |z| (bounded by 2u)."""
+    T = F.conv2d(mom.abs(), qw.abs(), groups=3) + qb.abs()[None, :, None, None]
+    tol_m = 9 * U32 * T[:, :12] + U32 * mean.abs()
+    tol_lv = 9 * U32 * T[:, 12:] + 8 * U32 * lv.abs()
+    std = torch.exp(0.5 * lv)
+    tol_z = tol_m + std * noise.abs() * (0.5 * tol_lv + 6 * U32) + 2 * U32 * z.abs()
+    return tol_m, tol_lv, tol_z
+
+
+def view_mean_tol(xv):
+    """ln3_view_mean_nhwc of xv (B, F, ...): an fp32 sum over the F views in order, then one division by F, within
+    (F + 1) u sum|x| / F of the float64 mean."""
+    F_ = xv.shape[1]
+    return (F_ + 1) * U32 * xv.double().abs().sum(1) / F_
+
+
+def _chunk_mean(h, num_frames):
+    """torch.chunk(N // num_frames) + mean(dim=0) per chunk, as the reference pools, in the kernel's summation order.  The
+    division is by a tensor: torch's CUDA division by a Python scalar multiplies by its reciprocal instead."""
+    outs = []
+    for f in h.chunk(h.shape[0] // num_frames):
+        s = f[0].clone()
+        for v in range(1, f.shape[0]):
+            s = s + f[v]
+        outs.append((s / torch.full_like(s, f.shape[0]))[None])
+    return torch.cat(outs)

@@ -16,10 +16,11 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from kernel_bounds import _swish_tol, attn_reference, conv_reference, gn_reference, pet_reference
+
 pytestmark = pytest.mark.gpu
 U = 2.0 ** -24
 PAD = 1024                # guard elements before and after every output
-SWISH_SLOPE = 1.1         # max |d/dz z sigmoid(z)| = 1.0998
 
 
 @pytest.fixture(scope="module")
@@ -66,61 +67,7 @@ def _check(got, ref, tol, what):
     return ratio
 
 
-def _expf_rel(z):
-    """__expf(x) error relative to exp(x): at most 2 + floor(|1.173 x|) ulp (CUDA programming guide), an ulp <= 2u."""
-    return (2 + torch.floor(1.173 * z.abs())) * 2 * U
-
-
-def _swish_tol(z, dz):
-    """Error of the kernel's v / (1 + __expf(-v)) with v = z + dz (|dz| the error of the fp32 pre-activation):
-    the input error passes with slope <= 1.1; __expf(-v) is off by _expf_rel relative, which moves 1 + e and so the
-    quotient by at most that much relative; the add and the division round once each (2u).  Below z = -88.7
-    __expf(-v) overflows to inf and the kernel returns -0: the whole value |s| is lost there (and is < 3e-37), and the
-    2^-126 floor covers quotients that fall into the subnormal range."""
-    s = z * torch.sigmoid(z)
-    rel = torch.where(z < -80, torch.ones_like(z), _expf_rel(z) + 3 * U)
-    return s, SWISH_SLOPE * dz + s.abs() * rel + 2.0 ** -126
-
-
 # ------------------------------------------------------------------ ln3_conv_nhwc
-def conv_reference(x, w, b, *, ksize, up, sc=None, sh=None, swish=False, res=None, tf32=False, dz=None):
-    """(ref, tol) in float64, NCHW.  x fp32 NHWC (N, Hin, Win, Cin) on the device; sc, sh fp32 (N, Cin) are the very
-    values the kernel gets, so the reference input is x_hat = swish(x sc + sh) evaluated in float64 and this isolates
-    the conv.  Per output element, with T = conv(|x_hat|, |w|) + |b| and K = ksize^2 Cin:
-      fp32: a chain of K fmaf plus the bias add: (K + 4) u T;
-      TF32: both operands rounded to nearest 10-bit mantissas (2^-11 relative each) before the fp32-accumulated
-            mma: 2^-10 T more;
-      input: the kernel's x_hat is off by d = u |z| (the fmaf z = x sc + sh rounds once), passed through swish by
-            _swish_tol, and the conv carries d through |w|: conv(d, |w|) (times 1 + 2^-9 for the TF32 rounding of
-            the perturbed value);
-      residual: the final add rounds once more, u |out|.
-    dz (N, Hin, Win, Cin) adds an upstream error of z (the composed GroupNorm test)."""
-    x64 = x.double()
-    d = torch.zeros_like(x64)
-    if sc is not None:
-        z = x64 * sc.double()[:, None, None, :] + sh.double()[:, None, None, :]
-        d = U * z.abs() + (dz if dz is not None else 0.0)
-        if swish:
-            xh, d = _swish_tol(z, d)
-        else:
-            xh = z
-    else:
-        xh = x64
-    xh, d = xh.permute(0, 3, 1, 2), d.permute(0, 3, 1, 2)
-    if up:
-        xh, d = F.interpolate(xh, scale_factor=2.0, mode="nearest"), F.interpolate(d, scale_factor=2.0, mode="nearest")
-    w64 = w.double()
-    pad = ksize // 2
-    ref = F.conv2d(xh, w64, None if b is None else b.double(), padding=pad)
-    T = F.conv2d(xh.abs(), w64.abs(), None if b is None else b.double().abs(), padding=pad)
-    K = ksize * ksize * x.shape[3]
-    tol = ((2.0 ** -10 if tf32 else 0.0) + (K + 4) * U) * T + (1 + 2.0 ** -9) * F.conv2d(d, w64.abs(), padding=pad)
-    if res is not None:
-        ref = ref + res.double().permute(0, 3, 1, 2)
-        tol = tol + U * ref.abs()
-    return ref, tol
-
-
 # (N, Hin, Win, Cin, Cout, ksize, upsample, gn, swish, bias, residual)
 DEC = {                                                    # the conv_sr tail of the VAE decoder
     "conv_in384": (16, 16, 384, 128, 3, False, False, False, True, False),
@@ -307,38 +254,6 @@ def _gn_call(x, gamma, beta, G, eps=1e-6):
     return outs[0]
 
 
-def gn_reference(x, gamma, beta, G, eps=1e-6):
-    """(sc, sh, tol_sc, tol_sh, e_mu, mu) in float64, each (N, C).  The kernel, per (image, group) of cnt = HW C/G
-    elements: each of 256 threads adds m = ceil(cnt / 256) terms in sequence, then a 5-level shuffle tree in each warp
-    and a 5-level tree over the 8 warp sums, so every term meets at most m + 10 roundings; the mean divides once more:
-      e_mu  <= (m + 11) u A,   A = sum |x| / cnt.
-    The second pass adds fmaf(d, d, q) of d = fl(x - mu_hat) (2u relative on d^2) over the same m + 10 levels, and
-    sum (x - mu_hat)^2 = sum (x - mu)^2 + cnt e_mu^2, so with var = biased variance
-      |var_hat - var| <= (m + 13) u var + e_mu^2        (the division by cnt included).
-    var + eps rounds (u) and rsqrtf is within 2 ulp (4u), so rstd is off by rel_r = 1/2 rel(var + eps) + 4u; then
-      sc = fl(gamma rstd):               |d sc| <= |sc| (rel_r + u)
-      sh = fl(beta - fl(mu_hat sc_hat)): |d sh| <= |sc| e_mu + |mu| |d sc| + u |mu sc| + u |sh|
-    every term taken 1 % larger for the second-order products."""
-    N, H, W, Cc = x.shape
-    cpg, cnt = Cc // G, H * W * Cc // G
-    m = -(-cnt // 256)
-    xg = x.double().reshape(N, H * W, G, cpg)
-    mu = xg.mean(dim=(1, 3))                                             # (N, G)
-    var = ((xg - mu[:, None, :, None]) ** 2).mean(dim=(1, 3))
-    A = xg.abs().mean(dim=(1, 3))
-    e_mu = 1.01 * (m + 11) * U * A
-    e_var = 1.01 * ((m + 13) * U * var + e_mu ** 2)
-    rstd = 1 / torch.sqrt(var + eps)
-    rel_r = 1.01 * (0.5 * (e_var / (var + eps) + U) + 4 * U)
-    rep = lambda t: t.repeat_interleave(cpg, dim=1)                      # (N, G) -> (N, C)
-    g64, b64 = gamma.double()[None], beta.double()[None]
-    sc = g64 * rep(rstd)
-    sh = b64 - rep(mu) * sc
-    tol_sc = 1.01 * sc.abs() * (rep(rel_r) + U)
-    tol_sh = 1.01 * (sc.abs() * rep(e_mu) + rep(mu).abs() * tol_sc + U * (rep(mu) * sc).abs() + U * sh.abs())
-    return sc, sh, tol_sc, tol_sh, rep(e_mu), rep(mu)
-
-
 def _gn_operands(N, H, W, Cc, G, seed, dc=0.0):
     g = torch.Generator().manual_seed(seed)
     x = torch.randn(N, H, W, Cc, generator=g) * (0.5 + torch.rand(N, 1, 1, Cc, generator=g))
@@ -422,51 +337,6 @@ def test_groupnorm_then_conv_composed(dev, N, Hin, Win, Cin, Cout, G, dc, tf32):
 
 
 # ------------------------------------------------------------------ ln3_attn_single_head
-KB = 32   # keys per block
-
-
-def attn_reference(q, k, v):
-    """(y, tol) in float64, (N, L, C).  The kernel pre-multiplies q by scale = fl(1 / sqrtf(C)) (scale 2u off the exact
-    C^-1/2, the product one more rounding), scores s_j with a C-term fmaf chain, so with a_j = C^-1/2 sum |q k_j|
-      |d s_j| <= (C + 4) u a_j;
-    p_j = __expf(fl(s_j - m)) with m the running max of the scores: the subtraction rounds (u |s_j - m|) and __expf adds
-    _expf_rel(s_j - m).  Shifting every score by the same m does not change the ratio, so m's own error drops out, and
-    |s_j - m| is largest with the final m, which the reference uses.  When a block raises the running max from m_old to
-    m_new, the kernel multiplies the numerator and the denominator accumulated so far by alpha = __expf(fl(m_old - m_new)).
-    That scales the keys already seen against the later ones, so alpha's own error is charged to each earlier key: key j
-    sees at most nb - 1 such rescales (nb = ceil(L / 32)), each with |m_old - m_new| <= m - s_j + 2 d_max (m_old >= s_j
-    since key j is already in, m_new <= m; d_max = the largest |d s|), so each is off by at most
-      eps_j = expm1(u r_j) + _expf_rel(r_j),  r_j = |s_j - m| + 2 d_max.
-    P stays fp32, so the relative error of the kernel's weight of key j is
-      e_j   = (1 + expm1((C + 4) u a_j + u |s_j - m|) + _expf_rel(s_j - m)) (1 + eps_j)^(nb - 1) - 1
-            (1 below -80, where ex2.approx flushes to 0)
-      num   |d num| <= sum_j p_j |v_j| e_j + n_acc 2u sum_j p_j |v_j| (1 + e_j)
-      den   |d l|   <= sum_j p_j e_j + n_acc 2u sum_j p_j (1 + e_j)
-      n_acc = L + 2 ceil(L / 32): one add per key (the 5-level block sum adds only the block's keys), one rescale
-              product per 32-key block in each accumulator
-      y     (|d num| + |y| |d l|) / (l - |d l|) + 2u |y| (1 / l and the product)."""
-    N, L, Cc = q.shape
-    q64, k64, v64 = q.double(), k.double(), v.double()
-    sc = Cc ** -0.5
-    s = (q64 @ k64.transpose(1, 2)) * sc
-    a = (q64.abs() @ k64.abs().transpose(1, 2)) * sc
-    m = s.amax(-1, keepdim=True)
-    p = torch.exp(s - m)
-    arg = (s - m).abs()
-    nb = math.ceil(L / KB)
-    r = arg + 2 * (Cc + 4) * U * a.amax(-1, keepdim=True)
-    eps = torch.expm1(U * r) + _expf_rel(r)
-    e = (1 + torch.expm1((Cc + 4) * U * a + U * arg) + _expf_rel(arg)) * (1 + eps) ** (nb - 1) - 1
-    e = torch.where(arg > 80, torch.ones_like(e), e)
-    n_acc = L + 2 * nb
-    l = p.sum(-1, keepdim=True)
-    y = (p @ v64) / l
-    d_num = (p * e) @ v64.abs() + n_acc * 2 * U * ((p * (1 + e)) @ v64.abs())
-    d_den = (p * e).sum(-1, keepdim=True) + n_acc * 2 * U * (p * (1 + e)).sum(-1, keepdim=True)
-    tol = (d_num + y.abs() * d_den) / (l - d_den) + 2 * U * y.abs()
-    return y, tol
-
-
 def _attn_call(q, k, v):
     """ln3_attn_single_head through the C ABI into a guarded buffer; two launches."""
     from ln3diff_b200 import _lib
@@ -542,27 +412,6 @@ def test_attn_single_head_rejects_unsupported_width(dev):
 
 
 # ------------------------------------------------------------------ ln3_patch_embed_triplane
-def pet_reference(lat, w, b, in_mul):
-    """(tokens, tol_tok, silu, tol_silu) in float64.  The kernel input is fl(lat in_mul), the same rounding torch does
-    for `lat * in_mul`, so the reference starts from that fp32 product.  Each token is a chain of K = 4 Cz fmaf
-    started from the bias: |d tok| <= (4 Cz + 2) u T, T = sum |w x| + |b|.  The bf16 copy is
-    fl_bf16(silu_k(tok_hat)): swish of a value off by d tok (_swish_tol), then round to nearest bf16: half an ulp of
-    8 significant bits, up to 2^-8 |silu| just above a power of two (+ 2^-8 of its error, and half the 2^-133 spacing
-    below bf16's normal range)."""
-    B, C3, S, _ = lat.shape
-    Cz, E = C3 // 3, w.shape[0] // 3
-    x = (lat * in_mul).double()                                       # fp32 product, as torch rounds it
-    w64 = w.double()
-    y = F.conv2d(x, w64, None if b is None else b.double(), stride=2, groups=3)
-    T = F.conv2d(x.abs(), w64.abs(), None if b is None else b.double().abs(), stride=2, groups=3)
-    tok = lambda t: t.reshape(B, E, 3, S // 2, S // 2).flatten(2).transpose(1, 2)     # B (3 h w) E
-    y, T = tok(y), tok(T)
-    tol = (4 * Cz + 2) * U * T
-    silu, tol_s = _swish_tol(y, tol)
-    tol_s = tol_s * (1 + 2.0 ** -8) + 2.0 ** -8 * silu.abs() + 2.0 ** -134
-    return y, tol, silu, tol_s
-
-
 def _pet_call(lat, w, b, in_mul, want_silu):
     """ln3_patch_embed_triplane through the C ABI into guarded buffers; two launches."""
     from ln3diff_b200 import _lib

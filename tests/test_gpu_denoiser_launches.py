@@ -28,15 +28,13 @@ layer and the worst element.  Finally the CUDA-graph replay of the same forward 
 audited eager forward."""
 from __future__ import annotations
 
-import collections
-import contextlib
-
-import numpy as np
 import pytest
 import torch
 
 import kernel_bounds as kb
 import mv23d_oracle as mo
+from launch_audit import FMHA_FACTOR, Step, _report, traced
+from launch_audit import Audit as LaunchAudit
 
 pytestmark = pytest.mark.gpu
 
@@ -51,9 +49,6 @@ ACT_GELU_ERF, ACT_GELU_TANH, ACT_SILU = 1, 2, 3
 # relative.  A slip of an fp8 check kind therefore cannot move its elements by 100x the bound; it must still put the
 # median affected element outside it (the check then fails on most of them), with margin.
 FP8_FACTOR = 2.0
-# The attention bound carries the bf16 rounding of P, 2^-8 of sum p |v| / l, which under diffuse attention over
-# ~800 keys is a few percent of |y|: a wrong K/V source moves the output by 20-90x that bound, not 100x.
-FMHA_FACTOR = 20.0
 
 
 @pytest.fixture(scope="module")
@@ -133,8 +128,6 @@ def inputs(family, layout, dev, seed=5):
 
 
 # ------------------------------------------------------------------ the expected launch sequence
-Step = collections.namedtuple("Step", "op kind layer")
-
 CONTEXT = {   # the cached conditioning of a context: (op, step) model-level, and per layer
     "t23d": ([("norm_modulate", "ctx_cast"), ("gemm", "ctx_fc1"), ("gemm", "ctx_fc2"), ("gemm", "ctx_kv_all")], []),
     "t23d_pixart": ([("norm_modulate", "cap_ln"), ("gemm", "cap")],
@@ -176,23 +169,12 @@ def expected_launches(family, depth, fp8, rows, split, mod_row=False):
 
 
 # ------------------------------------------------------------------ the auditor
-def _desc(v):
-    if isinstance(v, torch.Tensor):
-        return f"{tuple(v.shape)}/{tuple(v.stride())}+{v.storage_offset()} {str(v.dtype)[6:]}"
-    return repr(v) if not isinstance(v, (tuple, list)) else "(" + ", ".join(_desc(a) for a in v) + ")"
-
-
-def _clone(v):
-    if isinstance(v, tuple):
-        return tuple(_clone(a) for a in v)
-    return v.clone() if isinstance(v, torch.Tensor) else v
-
-
-class Audit:
+class Audit(LaunchAudit):
     """Checks each launch as it happens (block by block: only the values later launches read are kept)."""
 
     def __init__(self, m, family, seq, x, t, ctx, in_scale, rows, split, table_t=None, table_row=None):
-        self.m, self.family, self.seq = m, family, seq
+        super().__init__(seq)
+        self.m, self.family = m, family
         self.D, self.T, self.H, self.depth = m.embed_dim, m.pos_embed.shape[1], m.num_heads, m.depth
         self.M = B * self.T
         self.dev = x.device
@@ -207,11 +189,6 @@ class Audit:
         self.rec = {}
         self.kv, self.dkv, self.oc = {}, {}, {}
         self.wcache = {}
-        self.n_traced = self.n_checked = 0
-        self.ratio = collections.defaultdict(float)     # step kind -> max error / bound
-        self.sep = {}                                   # check kind -> median slip / bound
-        self.step = None
-        self.args_desc = ""
 
     # ---- weights from the module, rounded as the precision contract says
     def bf(self, p):
@@ -256,32 +233,6 @@ class Audit:
         return self.mod(l)[:, j * self.D:(j + 1) * self.D]
 
     # ---- assertions
-    def fail_msg(self, what, got, ref, bound, bad):
-        score = torch.where(bad, ((got - ref).abs() / bound.clamp_min(1e-300)).nan_to_num(float("inf")),
-                            torch.zeros_like(ref))
-        i = tuple(int(v) for v in np.unravel_index(int(score.flatten().argmax()), tuple(ref.shape)))
-        s = self.step
-        return (f"step {s.kind} layer {s.layer} ({what}): {int(bad.sum())} of {ref.numel()} elements out of bound; "
-                f"worst at index {i}: got {got[i].item()!r} expected {ref[i].item()!r} bound {bound[i].item():.3e}; "
-                f"launch args {self.args_desc}")
-
-    def within(self, what, got, ref, bound):
-        got = got.to(torch.float64)
-        bound = bound.to(torch.float64).expand_as(ref)
-        assert got.shape == ref.shape, (self.step, what, got.shape, ref.shape)
-        err = (got - ref).abs()
-        bad = ~(err <= bound)                        # NaN counts as out of bound
-        if bool(bad.any()):
-            raise AssertionError(self.fail_msg(what, got, ref, bound, bad))
-        r = float((err / bound.clamp_min(1e-300)).max())
-        key = self.step.kind
-        self.ratio[key] = max(self.ratio[key], r)
-
-    def separated(self, kind, ref, wrong, bound, affected=None, factor=100.0):
-        if kind not in self.sep:
-            self.sep[kind] = kb.assert_sensitive(f"{self.step.kind} layer {self.step.layer}: {kind}", ref, wrong,
-                                                 bound, affected, factor)
-
     def check_x(self, got, ref):
         """fp32 residual stream: at most 1 ulp (double-rounding ties only), bit-exact almost everywhere."""
         self.within("residual stream x", got, ref, kb.ulp_f32(ref))
@@ -373,17 +324,6 @@ class Audit:
             self.separated("norm_modulate_fp8 output" if self.fp8 else "norm_modulate output", y, wrong, bound_y,
                            factor=FP8_FACTOR if self.fp8 else 100.0)
         return y
-
-    # ---- the launch
-    def launch(self, i, op, args, kw, ret):
-        self.n_traced += 1
-        assert i < len(self.seq), f"launch {i} ({op}) beyond the {len(self.seq)} expected launches"
-        self.step = st = self.seq[i]
-        assert op == st.op, f"launch {i}: expected {st.op} ({st.kind} layer {st.layer}), traced {op}"
-        self.args_desc = ", ".join([_desc(a) for a in args] + [f"{k}={_desc(v)}" for k, v in kw.items()
-                                                              if v is not None])
-        getattr(self, "do_" + st.kind)(st.layer, args, kw, _clone(ret))
-        self.n_checked += 1
 
     # ---- context
     def do_ctx_cast(self, l, args, kw, ret):
@@ -780,33 +720,6 @@ class Audit:
         self.rec["out"] = ret
 
 
-# ------------------------------------------------------------------ the tracer
-@contextlib.contextmanager
-def traced(audit, monkeypatch, slip=None):
-    """Wraps the ops the denoisers call; `slip` = (kind, layer, fn(args, kw) -> (args, kw)) rewrites the arguments of
-    that one launch before it runs (a seeded host-side mapping error)."""
-    from ln3diff_b200 import ops
-    counter = [0]
-
-    def wrap(name, fn):
-        def w(*args, **kw):
-            i = counter[0]
-            counter[0] += 1
-            st = audit.seq[i] if i < len(audit.seq) else None
-            if slip is not None and st is not None and (st.kind, st.layer) == slip[:2]:
-                args, kw = slip[2](list(args), dict(kw))
-            ret = fn(*args, **kw)
-            audit.launch(i, name, args, kw, ret)
-            return ret
-        return w
-
-    with monkeypatch.context() as mp:
-        for name in TRACED:
-            mp.setattr(ops, name, wrap(name, getattr(ops, name)))
-        yield
-    assert counter[0] == len(audit.seq), f"traced {counter[0]} launches, expected {len(audit.seq)}"
-
-
 # ------------------------------------------------------------------ one audited forward
 def run_audit(family, prec, variant, dev, monkeypatch, slip=None, graph=True):
     m = model(family, dev)
@@ -824,7 +737,7 @@ def run_audit(family, prec, variant, dev, monkeypatch, slip=None, graph=True):
     seq = expected_launches(family, m.depth, prec == "fp8", rows, split, mod_row)
     table_t = torch.tensor([12.0, 250.0, 603.0, 871.0], device=dev) if mod_row else None
     audit = Audit(m, family, seq, x, t, ctx, in_scale, rows, split, table_t=table_t, table_row=2)
-    with torch.no_grad(), traced(audit, monkeypatch, slip):
+    with torch.no_grad(), traced(audit, monkeypatch, TRACED, slip):
         if mod_row:
             table = m.modulation_table(table_t)
             cx = m._context(ctx)
@@ -852,13 +765,6 @@ def run_audit(family, prec, variant, dev, monkeypatch, slip=None, graph=True):
 
 FAMILIES = ["t23d", "t23d_pixart", "i23d", "mv23d"]
 VARIANTS = ["cond-zero", "zero-cond", "distinct", "no-split", "full-attention"]
-
-
-def _report(audit, what):
-    print(f"\n{what}: {len(audit.seq)} launches checked; max error / bound per step:")
-    for k in sorted(audit.ratio):
-        print(f"    {k:24s} {audit.ratio[k]:.3e}")
-    print("  separation (median slip / bound): " + ", ".join(f"{k} {v:.3g}" for k, v in sorted(audit.sep.items())))
 
 
 @pytest.mark.parametrize("variant", VARIANTS)

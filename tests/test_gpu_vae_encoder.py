@@ -10,6 +10,7 @@ import torch
 import torch.nn.functional as F
 
 import vae_encoder_oracle as vo
+from kernel_bounds import _posterior_tol, downsample_reference
 
 pytestmark = pytest.mark.gpu
 U = 2.0 ** -24
@@ -63,11 +64,7 @@ def _golden_decoder(dev, arch="DiT2-S/2"):
 ])
 @pytest.mark.parametrize("tf32", [False, True])
 def test_downsample_elementwise(dev, N, H, W, Cin, Cout, tf32):
-    """Against F.conv2d(F.pad(x, (0,1,0,1)), stride=2) in float64.  Per element, with T = sum |w x| + |b| over the
-    K = 9 Cin terms:
-      fp32: a chain of K fused multiply-adds plus the bias add, |err| <= (K + 4) 2^-24 T;
-      TF32: both operands rounded to 10-bit mantissas (relative 2^-11 each, so 2^-10 per product) on top of the
-            fp32 accumulation: |err| <= (2^-10 + (K + 4) 2^-24) T."""
+    """Against F.conv2d(F.pad(x, (0,1,0,1)), stride=2) in float64, within kernel_bounds.downsample_reference's bound."""
     from ln3diff_b200 import ops
     g = torch.Generator().manual_seed(N * 1000 + H + Cin + Cout)
     x = torch.randn(N, H, W, Cin, generator=g)
@@ -86,10 +83,7 @@ def test_downsample_elementwise(dev, N, H, W, Cin, Cout, tf32):
     assert bool(buf[:pad].isnan().all()) and bool(buf[pad + n_out:].isnan().all())
     assert not bool(out.isnan().any())
     xc = x.to(dev, torch.float64).permute(0, 3, 1, 2)
-    ref = F.conv2d(F.pad(xc, (0, 1, 0, 1)), w.to(dev, torch.float64), b.to(dev, torch.float64), stride=2)
-    T = F.conv2d(F.pad(xc.abs(), (0, 1, 0, 1)), w.to(dev, torch.float64).abs(), stride=2) + b.abs().to(dev).double()[:, None, None]
-    K = 9 * Cin
-    tol = ((2.0 ** -10 if tf32 else 0.0) + (K + 4) * U) * T
+    ref, tol = downsample_reference(x.to(dev), w.to(dev), b.to(dev), tf32)
     err = (out.double().permute(0, 3, 1, 2) - ref).abs()
     assert bool((err <= tol).all()), float((err / tol).max())
     # the pad is on the bottom / right only: a one-pixel shift of the input moves the result far beyond the bound
@@ -99,19 +93,6 @@ def test_downsample_elementwise(dev, N, H, W, Cin, Cout, tf32):
 
 
 # ------------------------------------------------------------------ ln3_vae_posterior
-def _posterior_tol(qw, qb, mom, mean, lv, z, noise):
-    """Float64 vs kernel (an ulp is at most 2^-23 = 2u of the value).  Moments: an 8-term fmaf chain plus the bias add,
-    <= 9u T (T = sum |w h| + |b|).  logvar: the input error passes tanh with slope <= 1; div (1/2 ulp), tanhf (2 ulp)
-    and mul (1/2 ulp) add 3 ulp <= 6u |lv|, bounded by 8u.  std = exp(0.5 lv): 0.5 lv is exact, so a relative error of
-    0.5 err(lv) + 2 ulp (expf) = 0.5 err(lv) + 4u; the product std * noise adds u, the final sum u |z| (bounded by 2u)."""
-    T = vo.conv_terms_abs(mom, qw, pad=(0, 0, 0, 0), groups=3) + qb.abs()[None, :, None, None]
-    tol_m = 9 * U * T[:, :12] + U * mean.abs()
-    tol_lv = 9 * U * T[:, 12:] + 8 * U * lv.abs()
-    std = torch.exp(0.5 * lv)
-    tol_z = tol_m + std * noise.abs() * (0.5 * tol_lv + 6 * U) + 2 * U * z.abs()
-    return tol_m, tol_lv, tol_z
-
-
 def test_vae_posterior_elementwise_and_channel_mapping(dev):
     from ln3diff_b200 import ops
     g = torch.Generator().manual_seed(51)

@@ -10,6 +10,7 @@ import torch
 
 import test_gpu_render_conformance as rc
 import vae_encoder_oracle as vo
+from kernel_bounds import _chunk_mean, view_mean_tol
 from oracle import fixtures as fx
 from oracle import render as orender
 from test_vae_xl_host import NUM_FRAMES, dyna_encoder, xl_inputs
@@ -53,7 +54,7 @@ def test_view_mean_elementwise(dev, B, F, S, C):
         s = s + xv[:, f]
     assert torch.equal(got, s / F)
     ref = xv.double().mean(1)
-    tol = (F + 1) * U * xv.double().abs().sum(1) / F
+    tol = view_mean_tol(xv)
     assert bool(((got.double() - ref).abs() <= tol).all())
     assert torch.equal(ops.view_mean_nhwc(x.to(dev), F).cpu(), got)
 
@@ -102,18 +103,6 @@ def test_xl_encoder_vs_reference_golden(dev, golden, tf32):
     # the pooling is the mean of the per-view trunk outputs (not a sum, not one view)
     per_view = enc._trunk_nhwc(x, NUM_FRAMES)
     assert torch.equal(enc.forward_nhwc(x), _chunk_mean(per_view, NUM_FRAMES))
-
-
-def _chunk_mean(h, num_frames):
-    """torch.chunk(N // num_frames) + mean(dim=0) per chunk, as the reference pools, in the kernel's summation order.  The
-    division is by a tensor: torch's CUDA division by a Python scalar multiplies by its reciprocal instead."""
-    outs = []
-    for f in h.chunk(h.shape[0] // num_frames):
-        s = f[0].clone()
-        for v in range(1, f.shape[0]):
-            s = s + f[v]
-        outs.append((s / torch.full_like(s, f.shape[0]))[None])
-    return torch.cat(outs)
 
 
 def test_xl_encoder_num_frames_argument_follows_the_reference(dev):
