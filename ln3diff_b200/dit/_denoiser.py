@@ -302,16 +302,22 @@ class DenoiserMixin:
         buffer), or the eager launch sequence under LN3_CUDA_GRAPH=0 / inside a caller's own capture."""
         if graphs_enabled() and not torch.cuda.is_current_stream_capturing():
             g = self._graph(x.shape[0], cx)
-            g.x.copy_(x)
-            g.t.copy_(t)
-            if g.in_scale is not None:
-                if in_scale is None:
-                    g.in_scale.fill_(1.0)
-                else:
-                    g.in_scale.copy_(in_scale)
+            g.load(x, t, 1.0 if in_scale is None else in_scale)
             g.replay()
             return g.out.clone()
         return self._forward_impl(x.float().contiguous(), t, cx, in_scale, None)
+
+    def step_forward(self, rows: int, context, t: torch.Tensor, in_scale=None) -> StepForward:
+        """The forwards of a sampling loop over a fixed `rows`-sample batch conditioned on `context`: write the batch
+        into `.x` (rows, 3C, S, S) fp32, then `(k)` runs step k's forward and returns the output buffer, which the
+        next call overwrites.  t (steps, rows) fp32: every step's timesteps; in_scale (steps, rows) or None (1.0):
+        every step's c_in, for the families that set `_ln3_fused_in_scale`.
+
+        Each step is a replay of the cached CUDA graph (`_graph`), or the eager launch sequence on `.x` under
+        LN3_CUDA_GRAPH=0 / inside a caller's own capture.  A graph replay of a family with `modulation_table` reads
+        one shared adaLN row per step, all steps' rows computed from t[:, 0] in one pass (every sample of a step
+        shares its timestep), unless LN3_SHARED_MODULATION=0."""
+        return StepForward(self, rows, context, t, in_scale)
 
     @torch.no_grad()
     def forward(self, x, timesteps=None, context=None, y=None, get_attr="", in_scale=None, **kwargs):
@@ -336,6 +342,38 @@ class DenoiserMixin:
         cond_eps, uncond_eps = torch.split(eps, len(eps) // 2, dim=0)
         half = uncond_eps + cfg_scale * (cond_eps - uncond_eps)
         return torch.cat([half, half], dim=0)
+
+
+class StepForward:
+    """See DenoiserMixin.step_forward."""
+
+    def __init__(self, den, rows, context, t, in_scale):
+        if den._prep is None:
+            den.prepare()
+        self.den, self.cx, self.t, self.in_scale = den, den._context(context), t, in_scale
+        self.g = self.mod = None
+        if graphs_enabled() and not torch.cuda.is_current_stream_capturing():
+            shared = hasattr(den, "modulation_table") and os.environ.get("LN3_SHARED_MODULATION", "1") != "0"
+            self.g = den._graph(rows, self.cx, shared)
+            if shared:
+                self.mod = den.modulation_table(t[:, 0])
+            if in_scale is None:
+                self.g.load(in_scale=1.0)
+            self.x = self.g.x
+        else:
+            self.x = torch.empty(rows, 3 * den.in_channels, den.input_size, den.input_size,
+                                 device=den.pos_embed.device, dtype=torch.float32)
+
+    def __call__(self, k: int) -> torch.Tensor:
+        in_scale = None if self.in_scale is None else self.in_scale[k]
+        if self.g is None:
+            return self.den._forward_impl(self.x, self.t[k], self.cx, in_scale, None)
+        if self.mod is not None:
+            self.g.load(mod=self.mod[k:k + 1], in_scale=in_scale)
+        else:
+            self.g.load(t=self.t[k], in_scale=in_scale)
+        self.g.replay()
+        return self.g.out
 
 
 class PixArtMixin(DenoiserMixin):

@@ -61,9 +61,9 @@ class ContextCache:
 
 class ForwardGraph:
     """One captured forward: static inputs `.x` (B,3C,S,S), `.t` (B,), `.in_scale` (B,), optional `.mod`
-    (1, (6L+2)·D) shared modulation row; static output `.out`; `.replay()`.  Plain attributes and a bound
-    method only -- no closure over `self`, so a dropped graph is freed by reference counting, never by a
-    cyclic-GC pass that could land inside a later capture."""
+    (1, (6L+2)·D) shared modulation row, written by `.load()`; static output `.out`; `.replay()`.  Plain
+    attributes and bound methods only -- no closure over `self`, so a dropped graph is freed by reference
+    counting, never by a cyclic-GC pass that could land inside a later capture."""
 
     __slots__ = ("graph", "x", "t", "in_scale", "mod", "out", "n_kernels", "cross_attention_rows", "key")
 
@@ -73,6 +73,21 @@ class ForwardGraph:
         self.n_kernels = 0
         self.cross_attention_rows = None
         self.key = None
+
+    def load(self, x=None, t=None, in_scale=None, mod=None) -> None:
+        """Write the inputs of the next replay into the static buffers; an input left None keeps its contents.
+        `in_scale` is a (B,) tensor or a number; a graph without an in_scale input ignores it."""
+        if x is not None:
+            self.x.copy_(x)
+        if t is not None:
+            self.t.copy_(t)
+        if mod is not None:
+            self.mod.copy_(mod)
+        if in_scale is not None and self.in_scale is not None:
+            if isinstance(in_scale, torch.Tensor):
+                self.in_scale.copy_(in_scale)
+            else:
+                self.in_scale.fill_(in_scale)
 
     def replay(self) -> None:
         self.graph.replay()

@@ -11,13 +11,23 @@ which is algebraically the reference's  D = x - sq*net;  x' = x + (x - cfg(D))/s
 """
 from __future__ import annotations
 
-import os
-
 import torch
 
 from . import ops
-from .dit._graph import graphs_enabled
 from .sgm.modules.diffusionmodules.discretizer import LegacyDDPMDiscretization
+
+
+def _quantise(sigma: torch.Tensor, table: torch.Tensor):
+    """DiscreteDenoiser(EpsScaling, 1000 idx) on float32 sigmas of any shape; `table` holds its ascending sigmas.
+    Returns (timestep index, quantised sigma, c_in), each of sigma's shape."""
+    sq = table[(sigma[..., None] - table).abs().argmin(-1)]      # sigma_to_idx, possibly_quantize_sigma
+    idx = (sq[..., None] - table).abs().argmin(-1)               # possibly_quantize_c_noise
+    return idx, sq, 1 / (sq ** 2 + 1.0) ** 0.5                   # EpsScaling's c_in
+
+
+def _cfg_context(c: dict, uc: dict) -> dict:
+    """VanillaCFG.prepare_inputs' context: cat((uc, c)) per tensor key, the other keys passed through."""
+    return {k: torch.cat((uc[k], c[k]), 0) if k in ("vector", "crossattn", "concat") else c[k] for k in c}
 
 
 @torch.no_grad()
@@ -26,12 +36,8 @@ def edm_cfg_tables(num_steps: int, scale: float, B: int, device, dtype=torch.flo
     order as the reference's scalar tensors)."""
     disc = LegacyDDPMDiscretization()
     sigmas = disc(num_steps, device="cpu")                       # (num_steps+1,), last = 0
-    table = disc(1000, do_append_zero=False, flip=True)          # ascending, DiscreteDenoiser.sigmas
     s = sigmas[:-1]
-    idx = (s[None, :] - table[:, None]).abs().argmin(dim=0)      # sigma_to_idx
-    sq = table[idx]                                              # quantised sigma
-    idx2 = (sq[None, :] - table[:, None]).abs().argmin(dim=0)    # possibly_quantize_c_noise
-    c_in = 1 / (sq ** 2 + 1.0) ** 0.5
+    idx2, sq, c_in = _quantise(s, disc(1000, do_append_zero=False, flip=True))
     r = (sigmas[1:] - s) / s                                     # dt / sigma
     w_u = r * sq * (1 - scale)
     w_c = r * sq * scale
@@ -55,11 +61,7 @@ _PLANS: dict = {}
 def _plan_eval(plan, step, sigma, coef, *, kind, hist=(), hist_write=None, noise=False, draw=False, x_out=True):
     """Append one denoiser evaluation at `sigma` (a float32 scalar tensor).  kind 'D': e is the guided denoised D;
     kind 'd': e is the derivative (x_eval - D) / sigma.  coef holds the update part (a, b, c, h0, h1, h2, s)."""
-    table = plan["_table"]
-    idx = (sigma - table).abs().argmin()                          # DiscreteDenoiser.sigma_to_idx
-    sq = table[idx]                                               # possibly_quantize_sigma
-    idx2 = (sq - table).abs().argmin()                            # possibly_quantize_c_noise
-    c_in = 1 / (sq ** 2 + 1.0) ** 0.5                             # EpsScaling
+    idx2, sq, c_in = _quantise(sigma, plan["_table"])
     g, sqd = plan["scale"], float(sq)
     if kind == "D":                                               # D = x_eval - sq net, CFG-combined
         k = (1.0, -sqd * (1 - g), -sqd * g)
@@ -160,11 +162,10 @@ def edm_sampler_plan(sampler: str, num_steps: int, scale: float, eta: float = 1.
 
 
 @torch.no_grad()
-def _sample_t23d_plan(model, randn, c, uc, plan, use_graph, noise):
+def _sample_t23d_plan(model, randn, c, uc, plan, noise):
     """The evaluation plan's loop: one DiT forward of the 2B CFG batch per entry (a graph replay), then one
     ln3_sampler_step that writes the state, both halves of the next forward's input and the history slot."""
     B, dev = randn.shape[0], randn.device
-    E = len(plan["evals"])
     if noise is not None and (tuple(noise.shape) != (plan["num_steps"],) + tuple(randn.shape) or not noise.is_cuda):
         raise ValueError(f"noise must be a CUDA tensor of shape {(plan['num_steps'],) + tuple(randn.shape)}")
     tabs = plan.setdefault("_device", {}).get((B, dev))
@@ -173,30 +174,14 @@ def _sample_t23d_plan(model, randn, c, uc, plan, use_graph, noise):
             t_idx=plan["t_idx"].to(dev)[:, None].repeat(1, 2 * B).contiguous(),
             c_in=plan["c_in"].to(dev)[:, None].repeat(1, 2 * B).contiguous(),
             coef=plan["coef"].to(dev)[:, None, :].repeat(1, B, 1).contiguous())
-    ctx = torch.cat((uc["crossattn"], c["crossattn"]), 0).contiguous()   # VanillaCFG order: (uc, c)
+    fw = model.step_forward(2 * B, _cfg_context(c, uc), tabs["t_idx"], tabs["c_in"])
     xs = (randn.float() * plan["init_scale"]).contiguous()
     slots = [torch.empty_like(xs) for _ in range(plan["n_slots"])]
-    graph = use_graph and graphs_enabled() and hasattr(model, "capture_graph")
-    if graph:
-        shared = hasattr(model, "modulation_table") and os.environ.get("LN3_SHARED_MODULATION", "1") != "0"
-        g = model.capture_graph(2 * B, ctx, shared_mod=shared)
-        mod_table = model.modulation_table(tabs["t_idx"][:, 0]) if shared else None
-        xin = g.x
-    else:
-        xin = torch.empty((2 * B,) + tuple(xs.shape[1:]), device=dev, dtype=torch.float32)
+    xin = fw.x
     xin[:B].copy_(xs)
     xin[B:].copy_(xs)
     for k, ev in enumerate(plan["evals"]):
-        if graph:
-            if shared:
-                g.mod.copy_(mod_table[k:k + 1])
-            else:
-                g.t.copy_(tabs["t_idx"][k])
-            g.in_scale.copy_(tabs["c_in"][k])
-            g.replay()
-            net = g.out
-        else:
-            net = model(xin, tabs["t_idx"][k], ctx, in_scale=tabs["c_in"][k])
+        net = fw(k)
         nz = None
         if ev["draw"]:
             nz = noise[ev["step"]] if noise is not None else torch.randn_like(xs)
@@ -209,12 +194,15 @@ def _sample_t23d_plan(model, randn, c, uc, plan, use_graph, noise):
 
 @torch.no_grad()
 def sample_t23d(model, randn: torch.Tensor, c: dict, uc: dict, num_steps: int = 250,
-                scale: float = 6.5, tables: dict | None = None, use_graph: bool = True,
+                scale: float = 6.5, tables: dict | None = None,
                 sampler: str = "EulerEDMSampler", eta: float = 1.0, s_noise: float = 1.0, order: int = 4,
                 noise: torch.Tensor | None = None, s_churn: float = 0.0) -> torch.Tensor:
     """randn (B, 12, 32, 32) fp32 on the GPU (the reference draws it on the CPU generator and moves
-    it, sgm_DiffusionEngine.py:395); c / uc = {'crossattn': (B, 77, ctx_dim)}.  Returns the
-    denoised latents (B, 12, 32, 32) fp32.
+    it, sgm_DiffusionEngine.py:395); c / uc = {'crossattn': (B, 77, ctx_dim)} (and 'vector' (B, ctx_dim) for the
+    PixArt-style denoiser).  Returns the denoised latents (B, 12, 32, 32) fp32.
+
+    Every denoiser evaluation is one forward of the 2B-sample CFG batch (uc rows first) through the model's
+    `step_forward`: a replay of its cached CUDA graph, or eager launches under LN3_CUDA_GRAPH=0.
 
     `sampler` is one of the reference's sgm class names (SAMPLERS): 'EulerEDMSampler' (the default, the
     engine's) or HeunEDMSampler, EulerAncestralSampler, DPMPP2SAncestralSampler, DPMPP2MSampler and
@@ -230,40 +218,19 @@ def sample_t23d(model, randn: torch.Tensor, c: dict, uc: dict, num_steps: int = 
         if tables is not None:
             raise ValueError("tables= holds Euler-EDM coefficients; it cannot be used with sampler=" + repr(sampler))
         plan = edm_sampler_plan(sampler, num_steps, scale, eta, s_noise, order)
-        return _sample_t23d_plan(model, randn, c, uc, plan, use_graph, noise)
+        return _sample_t23d_plan(model, randn, c, uc, plan, noise)
     if noise is not None:
         raise ValueError("EulerEDMSampler draws no noise; noise= is for the ancestral samplers")
     B = randn.shape[0]
     if tables is None:
         tables = edm_cfg_tables(num_steps, scale, B, randn.device)
-    ctx = torch.cat((uc["crossattn"], c["crossattn"]), 0).contiguous()   # VanillaCFG order: (uc, c)
-    x = (randn.float() * tables["init_scale"]).contiguous()
-    xa, xb = x, torch.empty_like(x)
-    if use_graph and graphs_enabled() and hasattr(model, "capture_graph"):
-        # one CUDA graph = one DiT forward of the 2B CFG batch; replayed every step.  The graph is cached on
-        # the model per launch-sequence shape: this call computes the prompt batch's step-invariant
-        # conditioning into the model's static buffers and captures only the first time a shape is seen.
-        # every sample of a step shares its timestep: the adaLN modulations of all steps in one pass
-        shared = hasattr(model, "modulation_table") and os.environ.get("LN3_SHARED_MODULATION", "1") != "0"
-        g = model.capture_graph(2 * B, ctx, shared_mod=shared)
-        mod_table = model.modulation_table(tables["t_idx"][:num_steps, 0]) if shared else None
-        for i in range(num_steps):
-            g.x[:B].copy_(xa)
-            g.x[B:].copy_(xa)
-            if shared:
-                g.mod.copy_(mod_table[i:i + 1])
-            else:
-                g.t.copy_(tables["t_idx"][i])
-            g.in_scale.copy_(tables["c_in"][i])
-            g.replay()
-            ops.sampler_affine_update(xa, tables["coef"][i], g.out[:B], g.out[B:], out=xb)
-            xa, xb = xb, xa
-        return xa.clone()
-    x2 = torch.empty((2 * B,) + tuple(x.shape[1:]), device=x.device, dtype=torch.float32)
+    fw = model.step_forward(2 * B, _cfg_context(c, uc), tables["t_idx"][:num_steps], tables["c_in"][:num_steps])
+    xa = (randn.float() * tables["init_scale"]).contiguous()
+    xb = torch.empty_like(xa)
     for i in range(num_steps):
-        x2[:B].copy_(xa)
-        x2[B:].copy_(xa)
-        net = model(x2, tables["t_idx"][i], ctx, in_scale=tables["c_in"][i])
+        fw.x[:B].copy_(xa)
+        fw.x[B:].copy_(xa)
+        net = fw(i)
         ops.sampler_affine_update(xa, tables["coef"][i], net[:B], net[B:], out=xb)
         xa, xb = xb, xa
     return xa
@@ -381,16 +348,9 @@ def sample_flow(model, c: dict, uc: dict, num_samples: int, seed: int = 42, num_
     if dev.type != "cuda":
         raise RuntimeError("sample_flow runs on CUDA only (no CPU fallback)")
     _check_sde_method(sde, sampling_method)
-    torch.manual_seed(seed)
     C = 3 * model.in_channels if model.roll_out else model.in_channels
-    zs = torch.randn(num_samples, C, model.input_size, model.input_size).to(dev).to(dtype).float()
-    ctx = {}
-    for k in c:
-        if k in ("vector", "crossattn", "concat"):
-            ctx[k] = torch.cat((c[k], uc[k]), 0).to(dev).to(dtype).float().contiguous()
-        else:
-            assert c[k] == uc[k]
-            ctx[k] = c[k]
+    zs = flow_batch_noise(1, num_samples, (C, model.input_size, model.input_size), seed).to(dev).to(dtype).float()
+    ctx = flow_batch_context(c, uc, dev, dtype)
     if sde is not None:
         return sample_flow_sde(model, zs, ctx, num_samples, num_steps, cfg_scale, sde)[0][:num_samples]
     fn = Sampler(create_transport(snr_type="lognorm")).sample_ode(sampling_method=sampling_method, num_steps=num_steps)

@@ -372,42 +372,16 @@ def _is_library_cfg(model) -> bool:
     return isinstance(owner, DenoiserMixin) and getattr(model, "__func__", None) is type(owner).forward_with_cfg
 
 
-class CfgForward:
-    """The raw forward of a library denoiser on a fixed 2R-row CFG batch through fixed buffers: write the input into
-    `.x`, call with the (2R,) fp32 time rows, read the output (conditional rows first).  A replay of the denoiser's
-    captured graph, or its eager launch sequence under LN3_CUDA_GRAPH=0."""
-
-    def __init__(self, den, context, rows: int, like: th.Tensor):
-        from ..dit._graph import graphs_enabled
-        if den._prep is None:
-            den.prepare()
-        self.den, self.cx = den, den._context(context)
-        self.g = None
-        if graphs_enabled() and not th.cuda.is_current_stream_capturing():
-            self.g = den._graph(rows, self.cx)
-            if self.g.in_scale is not None:
-                self.g.in_scale.fill_(1.0)
-            self.x = self.g.x
-        else:
-            self.x = th.empty((rows,) + tuple(like.shape[1:]), device=like.device, dtype=th.float32)
-
-    def __call__(self, t_rows: th.Tensor) -> th.Tensor:
-        if self.g is None:
-            return self.den._forward_impl(self.x, t_rows, self.cx)
-        self.g.t.copy_(t_rows)
-        self.g.replay()
-        return self.g.out
-
-
 def sde_fused(plan, den, init, context, cfg_scale, draw, record=None):
-    """Run `plan` (sde_plan) on the CUDA fp32 2R-row CFG state `init` around denoiser `den`: one forward and one
-    ln3_flow_sde_step per entry.  `draw(k)` returns step k's noise, a CUDA fp32 (2N, ...) draw (N divides R), and is
-    called once per step in step order; `record(x)` receives every returned state as a new tensor (and, with
-    last_step=None, the last one again).  Returns the final state buffer (2R rows)."""
+    """Run `plan` (sde_plan) on the CUDA fp32 2R-row CFG state `init` around denoiser `den`: one forward (the
+    denoiser's `step_forward`, conditional rows first) and one ln3_flow_sde_step per entry.  `draw(k)` returns step k's
+    noise, a CUDA fp32 (2N, ...) draw (N divides R), and is called once per step in step order; `record(x)` receives
+    every returned state as a new tensor (and, with last_step=None, the last one again).  Returns the final state
+    buffer (2R rows)."""
     from .. import ops
-    dev, rows = init.device, init.shape[0]
-    fw = CfgForward(den, context, rows, init)
-    t_rows = th.tensor([e["t"] for e in plan["evals"]], dtype=th.float32)[:, None].repeat(1, rows).to(dev)
+    rows = init.shape[0]
+    t_rows = th.tensor([e["t"] for e in plan["evals"]], dtype=th.float32)[:, None].repeat(1, rows).to(init.device)
+    fw = den.step_forward(rows, context, t_rows)
     state = th.empty_like(fw.x)
     hist = th.empty_like(fw.x) if plan["sampling_method"] == "Heun" else None
     noise, drawn = None, -1
@@ -419,7 +393,7 @@ def sde_fused(plan, den, init, context, cfg_scale, draw, record=None):
                alpha=plan["pre_sigma"], out=fw.x.view(2, P, noise.shape[0] // 2, -1))
     last = None
     for k, e in enumerate(plan["evals"]):
-        f = fw(t_rows[k])
+        f = fw(k)
         if e["noise"] is not None and e["noise"] > drawn:
             noise, drawn = draw(e["noise"]), e["noise"]
         x_out = state if record is None or not e["record"] else th.empty_like(state)

@@ -7,6 +7,7 @@
     (rel-L2 < 2e-2, the Euler pipeline's bound), the mirrored class on its fused CUDA path (< 1e-2), the eager
     launch sequence (bit-identical), the forward count per sampler, and the device generator's state after an
     ancestral run;
+  - the Euler loop on DiT-B/2 and DiT-PixelArt-B/2, bit-identical to a hand-written loop of public forwards;
   - DPM++ 2M with fp8 GEMMs against bf16 (rel-L2 < 0.1, the fp8 denoiser tests' limit)."""
 import pytest
 import torch
@@ -183,6 +184,36 @@ def test_euler_default_is_unchanged(dev, setup):
     with pytest.raises(ValueError, match="churn"):
         pipeline.sample_t23d(S["m"], S["x0"].to(dev), S["cd"], S["ucd"], STEPS, 6.5, sampler="HeunEDMSampler",
                              s_churn=1.0)
+
+
+@pytest.mark.parametrize("arch", ["DiT-B/2", "DiT-PixelArt-B/2"])
+def test_euler_is_a_loop_of_public_forwards(dev, arch):
+    """The Euler loop, bit for bit, as a hand-written loop of the model's public forward: per step the two halves of
+    the CFG input, model(x2, t_idx, ctx, in_scale=c_in), then the affine update.  DiT-B/2 runs its shared adaLN rows
+    in the pipeline; the PixArt-style denoiser has no such table and ignores in_scale."""
+    from ln3diff_b200 import ops, pipeline
+    from ln3diff_b200.utils import build_t23d
+    m = build_t23d(arch, device=dev)
+    B = 2
+    g = torch.Generator().manual_seed(17)
+    x0 = torch.randn(B, 12, 32, 32, generator=g).to(dev)
+    c = {"crossattn": torch.randn(B, 77, 768, generator=g).to(dev)}
+    if arch == "DiT-PixelArt-B/2":
+        c["vector"] = torch.randn(B, 768, generator=g).to(dev)
+    uc = {k: torch.zeros_like(v) for k, v in c.items()}
+    out = pipeline.sample_t23d(m, x0, c, uc, STEPS, 6.5)
+
+    tabs = pipeline.edm_cfg_tables(STEPS, 6.5, B, dev)
+    ctx = {k: torch.cat((uc[k], c[k])) for k in c}
+    x = x0 * tabs["init_scale"]
+    x2 = torch.empty(2 * B, 12, 32, 32, device=dev)
+    for i in range(STEPS):
+        x2[:B].copy_(x)
+        x2[B:].copy_(x)
+        net = m(x2, tabs["t_idx"][i], ctx, in_scale=tabs["c_in"][i])
+        x = ops.sampler_affine_update(x, tabs["coef"][i], net[:B], net[B:])
+    assert torch.isfinite(out).all()
+    assert torch.equal(out, x), _rel(out, x)
 
 
 @pytest.mark.parametrize("name", ANCESTRAL)
