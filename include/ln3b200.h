@@ -87,14 +87,16 @@ size_t ln3_gemm_workspace_bytes(void);
 int ln3_gemm_bf16(const ln3_gemm_args* args, void* stream);
 
 /* ------------------------------------------------------------------ attention (wgmma)
- * out[b, i, h*64:(h+1)*64] = softmax(q_h k_h^T * scale) v_h, no mask: replaces
+ * out[b, i, h*hd:(h+1)*hd] = softmax(q_h k_h^T * scale) v_h, no mask: replaces
  * xformers.ops.memory_efficient_attention at vit/vision_transformer.py:114-118 (packed qkv of
  * MemEffAttention), ldm/modules/attention.py:279-307 (cross-attention, incl. its three
  * permute+contiguous copies) and the DiT2 decoder attention (dit/dit_decoder.py).
- * q/k/v/out are bf16; head h of row i of batch b lives at ptr + b*bs + i*ld + h*64, so a packed
- * (B, N, 3, H, 64) qkv buffer is addressed as q = base, k = base + H*64, v = base + 2*H*64 with
- * ld = 3*H*64.  Lq and Lkv are arbitrary (tails are zero-filled by TMA and masked).
- * head_dim must be 64 (every registry entry on the path except DiT-XL, SURVEY.md appendix A).
+ * q/k/v/out are bf16; head h of row i of batch b lives at ptr + b*bs + i*ld + h*hd, so a packed
+ * (B, N, 3, H, hd) qkv buffer is addressed as q = base, k = base + H*hd, v = base + 2*H*hd with
+ * ld = 3*H*hd.  Lq and Lkv are arbitrary (tails are zero-filled by TMA and masked).
+ * head_dim (hd) is 64 (DiT-S/B/L, the PixArt denoisers, the DiT2 VAE, CLIP) or 72 (DiT-XL/2: 1152 / 16 heads);
+ * any other value returns LN3_EUNSUPPORTED.  At head_dim 72 a second K/V source (k2/v2) returns
+ * LN3_EUNSUPPORTED; causal works at both widths.  `scale` is the caller's (head_dim ** -0.5 in every model).
  */
 typedef struct ln3_fmha_args {
   const void* q;

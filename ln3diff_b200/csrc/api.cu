@@ -116,14 +116,15 @@ int make_tmap_3d_bf16(CUtensorMap* out, const void* ptr, long long d0, long long
                       long long s1, long long s2, int box0, int box1) {
   EncodeTiledFn fn = get_encode_fn();
   if (!fn) return LN3_ECUDA;
-  if (box0 != 64) return set_error(LN3_EINVAL, "tmap: box0 must be 64 (128B swizzle)");
+  if (box0 != 64 && box0 != 8) return set_error(LN3_EINVAL, "tmap: box0 must be 64 (128B swizzle) or 8 (no swizzle)");
   cuuint64_t dims[3] = {static_cast<cuuint64_t>(d0), static_cast<cuuint64_t>(d1),
                         static_cast<cuuint64_t>(d2)};
   cuuint64_t strides[2] = {static_cast<cuuint64_t>(s1) * 2, static_cast<cuuint64_t>(s2) * 2};
   cuuint32_t box[3] = {static_cast<cuuint32_t>(box0), static_cast<cuuint32_t>(box1), 1};
   cuuint32_t estr[3] = {1, 1, 1};
   CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(ptr), dims, strides,
-                  box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                  box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                  box0 == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE,
                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS)
     return set_error(LN3_ECUDA, "cuTensorMapEncodeTiled(3d %lldx%lldx%lld) -> %d", d2, d1, d0,

@@ -24,6 +24,11 @@ namespace {
 
 constexpr int BM = 128;
 constexpr int BN = 128;
+// Head width of the head-RMSNorm epilogue: whole heads per BN tile, weights [nsec][kHnHead].  The denoisers
+// with q/k norms all have 64-wide heads; DiT-XL/2's 72-wide heads carry none (TextCondDiTBlock), and the
+// host (ops.gemm / ops.gemm_fp8) refuses any other head_norm weight width.
+constexpr int kHnHead = 64;
+static_assert(BN % kHnHead == 0, "head-norm heads must tile BN");
 constexpr int BK = 128;  // 128 e4m3 = 128 bytes = one 128B-swizzle row
 constexpr int kStages = 6;
 constexpr int kABytes = BM * BK;  // 16 KB
@@ -70,8 +75,8 @@ __device__ __forceinline__ void epilogue(const Fp8Params& p, float* acc, int m_b
   if constexpr (EPI == kEpiBf16HeadNorm) {
     // a 64-column head of one row lives in the 4 lanes of a quad (16 values each); same arithmetic as the bf16 GEMM
 #pragma unroll
-    for (int h = 0; h < BN / 64; ++h) {
-      const int sec = (n_base + 64 * h) / p.hn_sec_cols;
+    for (int h = 0; h < BN / kHnHead; ++h) {
+      const int sec = (n_base + kHnHead * h) / p.hn_sec_cols;
       if (sec >= p.hn_nsec) continue;
       float s0 = 0.f, s1 = 0.f;
 #pragma unroll
@@ -83,8 +88,8 @@ __device__ __forceinline__ void epilogue(const Fp8Params& p, float* acc, int m_b
       s0 += __shfl_xor_sync(0xffffffffu, s0, 2);
       s1 += __shfl_xor_sync(0xffffffffu, s1, 1);
       s1 += __shfl_xor_sync(0xffffffffu, s1, 2);
-      const float r0 = rsqrtf(s0 * (1.0f / 64.0f) + p.hn_eps), r1 = rsqrtf(s1 * (1.0f / 64.0f) + p.hn_eps);
-      const float* w = p.hn_w + sec * 64;
+      const float r0 = rsqrtf(s0 * (1.0f / kHnHead) + p.hn_eps), r1 = rsqrtf(s1 * (1.0f / kHnHead) + p.hn_eps);
+      const float* w = p.hn_w + sec * kHnHead;
 #pragma unroll
       for (int i = 8 * h; i < 8 * h + 8; ++i) {
         const float2 ww = __ldg(reinterpret_cast<const float2*>(w + 8 * (i - 8 * h) + 2 * q));
@@ -286,8 +291,8 @@ int gemm_fp8(const ln3_gemm_fp8_args* a, cudaStream_t stream) {
                      a->act);
   }
   if (epi == kEpiBf16HeadNorm &&
-      (a->head_norm_nsec <= 0 || a->head_norm_sec_cols <= 0 || a->head_norm_sec_cols % 64 != 0))
-    return set_error(LN3_EINVAL, "gemm_fp8: head_norm sections must be positive multiples of 64 columns");
+      (a->head_norm_nsec <= 0 || a->head_norm_sec_cols <= 0 || a->head_norm_sec_cols % kHnHead != 0))
+    return set_error(LN3_EINVAL, "gemm_fp8: head_norm sections must be positive multiples of %d columns (the head width)", kHnHead);
 
   CUtensorMap ta, tb;
   int rc = make_tmap_2d_u8(&ta, a->A, a->M, a->K, a->lda, BM, BK);

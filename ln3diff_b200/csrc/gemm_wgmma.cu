@@ -29,6 +29,11 @@ namespace ln3 {
 static constexpr int BM = 128;
 static constexpr int BN = 128;
 static constexpr int BK = 64;  // 64 bf16 = 128 bytes = one 128B-swizzle row
+// Head width of the head-RMSNorm epilogue: whole heads per BN tile, weights [nsec][kHnHead].  The denoisers
+// with q/k norms all have 64-wide heads; DiT-XL/2's 72-wide heads carry none (TextCondDiTBlock), and the
+// host (ops.gemm / ops.gemm_fp8) refuses any other head_norm weight width.
+static constexpr int kHnHead = 64;
+static_assert(BN % kHnHead == 0, "head-norm heads must tile BN");
 static constexpr int kStages = 5;
 static constexpr int kABytes = BM * BK * 2;  // 16 KB
 static constexpr int kBBytes = BN * BK * 2;  // 16 KB
@@ -105,8 +110,8 @@ __device__ __forceinline__ void epilogue(const GemmParams& p, float* acc, int m_
   if constexpr (HN) {
     // a 64-column head of one row lives in the 4 lanes of a quad (16 values each)
 #pragma unroll
-    for (int h = 0; h < BN / 64; ++h) {
-      const int sec = (n_base + 64 * h) / p.hn_sec_cols;
+    for (int h = 0; h < BN / kHnHead; ++h) {
+      const int sec = (n_base + kHnHead * h) / p.hn_sec_cols;
       if (sec >= p.hn_nsec) continue;
       float s0 = 0.f, s1 = 0.f;
 #pragma unroll
@@ -118,8 +123,8 @@ __device__ __forceinline__ void epilogue(const GemmParams& p, float* acc, int m_
       s0 += __shfl_xor_sync(0xffffffffu, s0, 2);
       s1 += __shfl_xor_sync(0xffffffffu, s1, 1);
       s1 += __shfl_xor_sync(0xffffffffu, s1, 2);
-      const float r0 = rsqrtf(s0 * (1.0f / 64.0f) + p.hn_eps), r1 = rsqrtf(s1 * (1.0f / 64.0f) + p.hn_eps);
-      const float* w = p.hn_w + sec * 64;
+      const float r0 = rsqrtf(s0 * (1.0f / kHnHead) + p.hn_eps), r1 = rsqrtf(s1 * (1.0f / kHnHead) + p.hn_eps);
+      const float* w = p.hn_w + sec * kHnHead;
 #pragma unroll
       for (int i = 8 * h; i < 8 * h + 8; ++i) {
         const float2 ww = __ldg(reinterpret_cast<const float2*>(w + 8 * (i - 8 * h) + 2 * q));
@@ -398,8 +403,8 @@ int gemm_bf16(const ln3_gemm_args* a, cudaStream_t stream) {
   if (a->head_norm_w != nullptr) {
     if (a->out_kind != LN3_OUT_BF16 || a->act != LN3_ACT_NONE)
       return set_error(LN3_EINVAL, "gemm: head_norm needs LN3_OUT_BF16 and no activation");
-    if (a->head_norm_nsec <= 0 || a->head_norm_sec_cols <= 0 || a->head_norm_sec_cols % 64 != 0)
-      return set_error(LN3_EINVAL, "gemm: head_norm sections must be positive multiples of 64 columns");
+    if (a->head_norm_nsec <= 0 || a->head_norm_sec_cols <= 0 || a->head_norm_sec_cols % kHnHead != 0)
+      return set_error(LN3_EINVAL, "gemm: head_norm sections must be positive multiples of %d columns (the head width)", kHnHead);
     return launch_gemm<LN3_ACT_NONE, LN3_OUT_BF16, true>(ta, tb, to, p, stream);
   }
   if (a->act < LN3_ACT_NONE || a->act > LN3_ACT_QUICK_GELU) return set_error(LN3_EINVAL, "gemm: unknown activation %d", a->act);

@@ -61,7 +61,7 @@ inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
 int make_tmap_2d_bf16(CUtensorMap* out, const void* ptr, long long rows, long long cols,
                       long long ld, int box_rows, int box_cols);
 // 3-D bf16 tensor map: tensor [d2, d1, d0] (d0 contiguous) with element strides (s2, s1, 1),
-// box [1, box1, box0], 128-byte swizzle.
+// box [1, box1, box0], 128-byte swizzle for box0 = 64, none for box0 = 8 (rows of 16 bytes, packed).
 int make_tmap_3d_bf16(CUtensorMap* out, const void* ptr, long long d0, long long d1, long long d2,
                       long long s1, long long s2, int box0, int box1);
 

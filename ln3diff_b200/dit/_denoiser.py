@@ -73,11 +73,16 @@ def run_blocks(blocks: list, cx: dict, ws: dict, x2: torch.Tensor, mods, heads: 
     """Every block of one forward as a fixed launch sequence over the workspace `ws` (no host syncs, so it
     can be captured in a CUDA graph).  x2 (B·T, D) fp32 residual stream, updated in place; mods[l] (B, 6D) fp32:
     layer l's shift / scale / gate rows of the attention (0-2) and of the MLP (3-5).  cx: 'kv' [(k, v)] per layer,
-    (B, Lc, D) views; 'rows' / 'oconst' from `cross_attention_context`; optional 'dkv' [(k, v)] per layer, a
-    second self-attention K/V source."""
+    (B, Lc, E) views; 'rows' / 'oconst' from `cross_attention_context`; optional 'dkv' [(k, v)] per layer, a
+    second self-attention K/V source.  E, the cross-attention's inner width (heads x its head width), is D except
+    in DiT-XL/2, whose cross-attention keeps 64-wide heads (E = 1024) beside 72-wide self-attention heads; its
+    output then takes the first M·E elements of ws['att']."""
     M, D = x2.shape
     B = M // T
-    qkv3, att3, q3 = ws["qkv"].view(B, T, 3 * D), ws["att"].view(B, T, D), ws["q"].view(B, T, D)
+    E = blocks[0]["cq_w"].shape[0]
+    qkv3, att3, q3 = ws["qkv"].view(B, T, 3 * D), ws["att"].view(B, T, D), ws["q"].view(B, T, E)
+    attc = ws["att"].view(-1)[:M * E].view(M, E)
+    attc3 = attc.view(B, T, E)
     (g0, g1), oconst = cx["rows"], cx["oconst"]
     r0, r1 = g0 * T, g1 * T        # token rows that need real cross-attention
     # x += gate_msa * attn ; xb = bf16(x): the un-normalised query input of the cross-attention.  Only the
@@ -117,8 +122,8 @@ def run_blocks(blocks: list, cx: dict, ws: dict, x2: torch.Tensor, mods, heads: 
             ops.norm_modulate(x2, norm=NORM_NONE, out=ws["xb"], resid=val, resid_gate=sl(2), resid_gate_rows=T)
         if r1 > r0:
             ops.gemm(ws["xb"][r0:r1], W["cq_w"], out=ws["q"][r0:r1], head_norm=W.get("cq_norm"), head_norm_sec_cols=D)
-            ops.fmha(q3[g0:g1], k[g0:g1], v[g0:g1], heads, out=att3[g0:g1])
-            ops.gemm(ws["att"][r0:r1], W["co_w"], W["co_b"], out=val[r0:r1])
+            ops.fmha(q3[g0:g1], k[g0:g1], v[g0:g1], heads, out=attc3[g0:g1])
+            ops.gemm(attc[r0:r1], W["co_w"], W["co_b"], out=val[r0:r1])
         # x += cross_attn (no gate) ; a = modulate(norm(x)).  Identical-token samples take the closed form.
         norm_a(**_pre_norm(W, "n2_w"), shift=sl(3), scale=sl(4), mod_rows=T, resid=val,
                resid_bcast=oconst[l] if oconst is not None else None, resid_bcast_rows=T,
@@ -268,7 +273,8 @@ class DenoiserMixin:
             M = B * T
             e = lambda *s, dt=torch.bfloat16: torch.empty(*s, device=dev, dtype=dt)
             ws = self._ws[B] = dict(tfeat=e(B, 256), th=e(B, D), st=e(B, D), x=e(B, T, D, dt=torch.float32),
-                                    xb=e(M, D), a=e(M, D), v=e(M, D), qkv=e(M, 3 * D), att=e(M, D), q=e(M, D),
+                                    xb=e(M, D), a=e(M, D), v=e(M, D), qkv=e(M, 3 * D), att=e(M, D),
+                                    q=e(M, self.blocks[0].cross_attn.to_q.out_features),
                                     h=e(M, int(self.mlp_ratio) * D), **self._mod_workspace(B, e))
             if self.gemm_precision == "fp8":
                 H = int(self.mlp_ratio) * D

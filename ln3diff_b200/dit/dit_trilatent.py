@@ -35,8 +35,8 @@ class DiT_TriLatent(DenoiserMixin, nn.Module):
         assert roll_out, "DiT_TriLatent requires roll_out=True (dit_trilatent.py:49)"
         if patch_size != 2:
             raise NotImplementedError("libln3b200 implements patch_size=2 (every release config)")
-        if hidden_size // num_heads != 64:
-            raise NotImplementedError("libln3b200 attention implements head_dim=64 (DiT-S/B/L)")
+        if hidden_size % num_heads or hidden_size // num_heads not in (64, 72):
+            raise NotImplementedError("libln3b200 attention implements head_dim 64 (DiT-S/B/L) and 72 (DiT-XL)")
         if vit_blk is not TextCondDiTBlock:
             raise NotImplementedError("T23D path is built with vit_blk=TextCondDiTBlock "
                                       "(guided_diffusion/script_util.py:407-415)")
@@ -105,17 +105,18 @@ class DiT_TriLatent(DenoiserMixin, nn.Module):
         P = self._prep
         B, Lc, Cc = context.shape
         D = self.embed_dim
+        E = self.blocks[0].cross_attn.to_k.out_features   # 64 x heads: D, or 1024 for DiT-XL/2
         # Static, model-owned output buffers per (B, Lc): captured graphs read K/V and the closed-form rows
         # through raw pointers, so a new prompt batch rewrites them in place and replays the same graph.
         st = self._static((B, Lc), lambda: dict(
-            kv=torch.empty(B * Lc, self.depth * 2 * D, device=context.device, dtype=torch.bfloat16),
+            kv=torch.empty(B * Lc, self.depth * 2 * E, device=context.device, dtype=torch.bfloat16),
             oc=torch.empty(self.depth, B, D, device=context.device, dtype=torch.bfloat16)))
         c = context.reshape(B * Lc, Cc).float().contiguous()
         cb = ops.norm_modulate(c, norm=NORM_NONE)
         c1 = ops.gemm(cb, P["c1_w"], P["c1_b"], act=ops.ACT_GELU_TANH)
         c2 = ops.gemm(c1, P["c2_w"], P["c2_b"])
-        ops.gemm(c2, P["kv_w"], out=st["kv"])  # every layer's K|V in one GEMM: (B*Lc, depth*2*D)
-        kv = st["kv"].view(B, Lc, self.depth, 2, D)
+        ops.gemm(c2, P["kv_w"], out=st["kv"])  # every layer's K|V in one GEMM: (B*Lc, depth*2*E)
+        kv = st["kv"].view(B, Lc, self.depth, 2, E)
         kv = [(kv[:, :, l, 0], kv[:, :, l, 1]) for l in range(self.depth)]
         return self._ctx_cache.put((context,), cross_attention_context(kv, c2.view(B, Lc, -1), P["blocks"], st["oc"]))
 

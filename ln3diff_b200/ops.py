@@ -76,7 +76,7 @@ def gemm(a: torch.Tensor, w: torch.Tensor, bias: torch.Tensor | None = None, *,
     if head_norm is not None:
         _cuda(head_norm, "head_norm", torch.float32)
         _req(head_norm.dim() == 2 and head_norm.shape[1] == 64 and head_norm.is_contiguous(),
-             "head_norm must be contiguous (nsec, 64)")
+             "head_norm must be contiguous (nsec, 64): the head-RMSNorm epilogue normalises 64-wide heads only")
         args.head_norm_w, args.head_norm_nsec = head_norm.data_ptr(), head_norm.shape[0]
         args.head_norm_sec_cols, args.head_norm_eps = head_norm_sec_cols, head_norm_eps
     args.act, args.out_kind = act, out_kind
@@ -87,34 +87,38 @@ def gemm(a: torch.Tensor, w: torch.Tensor, bias: torch.Tensor | None = None, *,
 def fmha(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, heads: int, *,
          out: torch.Tensor | None = None, scale: float | None = None,
          k2: torch.Tensor | None = None, v2: torch.Tensor | None = None, causal: bool = False) -> torch.Tensor:
-    """softmax(q k^T * scale) v per head.  q (B,Lq,H*64), k/v (B,Lkv,H*64) bf16 views with unit
-    inner stride (slices of a packed qkv buffer are fine); returns (B,Lq,H*64) bf16.
+    """softmax(q k^T * scale) v per head.  q (B,Lq,H*hd), k/v (B,Lkv,H*hd) bf16 views with unit
+    inner stride (slices of a packed qkv buffer are fine), head width hd 64 or 72 (k2/v2 need 64);
+    returns (B,Lq,H*hd) bf16.  scale defaults to hd ** -0.5.
     causal=True: key j is visible to query i only when j <= i (CLIP text tower)."""
     for name, t in (("q", q), ("k", k), ("v", v)):
         _cuda(t, name, torch.bfloat16)
-        _req(t.dim() == 3 and t.stride(2) == 1, f"{name} must be (B,L,H*64) with unit inner stride")
+        _req(t.dim() == 3 and t.stride(2) == 1, f"{name} must be (B,L,H*head_dim) with unit inner stride")
     B, Lq, C_ = q.shape
-    _req(C_ == heads * 64, "head_dim must be 64")
+    _req(heads > 0 and C_ % heads == 0, "q's width must be heads * head_dim")
+    hd = C_ // heads
+    _req(hd in (64, 72), f"head_dim must be 64 or 72, got {hd}")
     _req(k.shape == v.shape and k.shape[0] == B and k.shape[2] == C_, "k/v shape mismatch")
     Lkv = k.shape[1]
     if out is None:
         out = torch.empty((B, Lq, C_), device=q.device, dtype=torch.bfloat16)
     _cuda(out, "out", torch.bfloat16)
-    _req(out.shape == (B, Lq, C_) and out.stride(2) == 1, "out must be (B,Lq,H*64)")
+    _req(out.shape == (B, Lq, C_) and out.stride(2) == 1, "out must be (B,Lq,H*head_dim)")
     a = _lib.FmhaArgs()
     a.q, a.k, a.v, a.out = q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr()
-    a.B, a.H, a.Lq, a.Lkv, a.head_dim = B, heads, Lq, Lkv, 64
+    a.B, a.H, a.Lq, a.Lkv, a.head_dim = B, heads, Lq, Lkv, hd
     a.q_ld, a.q_bs = q.stride(1), q.stride(0)
     a.k_ld, a.k_bs = k.stride(1), k.stride(0)
     a.v_ld, a.v_bs = v.stride(1), v.stride(0)
     a.o_ld, a.o_bs = out.stride(1), out.stride(0)
-    a.scale = float(scale if scale is not None else 64 ** -0.5)
+    a.scale = float(scale if scale is not None else hd ** -0.5)
     a.causal = 1 if causal else 0
     _req(not (causal and k2 is not None), "causal attention takes a single K/V source")
     if k2 is not None:
         for name, t in (("k2", k2), ("v2", v2)):
             _cuda(t, name, torch.bfloat16)
-            _req(t.dim() == 3 and t.stride(2) == 1 and t.shape[0] == B and t.shape[2] == C_, f"{name} must be (B,L2,H*64)")
+            _req(t.dim() == 3 and t.stride(2) == 1 and t.shape[0] == B and t.shape[2] == C_,
+                 f"{name} must be (B,L2,H*head_dim)")
         _req(k2.shape == v2.shape, "k2/v2 shape mismatch")
         a.k2, a.v2, a.Lkv2 = k2.data_ptr(), v2.data_ptr(), k2.shape[1]
         a.k2_ld, a.k2_bs, a.v2_ld, a.v2_bs = k2.stride(1), k2.stride(0), v2.stride(1), v2.stride(0)
@@ -322,7 +326,7 @@ def gemm_fp8(a_q: torch.Tensor, a_scale: torch.Tensor, w_q: torch.Tensor, w_scal
     if head_norm is not None:
         _cuda(head_norm, "head_norm", torch.float32)
         _req(head_norm.dim() == 2 and head_norm.shape[1] == 64 and head_norm.is_contiguous(),
-             "head_norm must be contiguous (nsec, 64)")
+             "head_norm must be contiguous (nsec, 64): the head-RMSNorm epilogue normalises 64-wide heads only")
         args.head_norm_w, args.head_norm_nsec = head_norm.data_ptr(), head_norm.shape[0]
         args.head_norm_sec_cols, args.head_norm_eps = head_norm_sec_cols, head_norm_eps
     args.act, args.out_kind = act, out_kind
