@@ -600,8 +600,8 @@ int ln3_pack_frames(const ln3_pack_frames_args* args, void* stream);
  *   (TF32 applies to ksize 3; ksize 1 always runs fp32), N < 0, non-positive H, W, Cin or Cout, upsample with odd
  *   H or W, only one of in_scale / in_shift, or a NULL x, w or out -- checked before N == 0 returns without a launch.
  * ln3_conv_cout_tile: the output channels per CTA (32 or 64) ln3_conv_nhwc takes for these dims: 32 when
- *   Cout < 64 or when 64-channel CTAs would give fewer than two per SM of the current device (64 regardless of
- *   the SM count when the environment sets LN3_CONV_COT64=1, read once per process); 0 for a non-positive argument.
+ *   Cout < 64 or when 64-channel CTAs would give fewer than two per SM of the current device; 0 for a
+ *   non-positive argument.
  * ln3_groupnorm_stats: torch.nn.GroupNorm(G, C, eps) statistics of x [N, HW, C] folded with the
  *   affine parameters into per-(image, channel) scale / shift [N, C].  N <= 0 returns without a launch;
  *   otherwise LN3_EINVAL for non-positive G, C or HW, C % G != 0, C / G > 256 or a NULL pointer.

@@ -3,8 +3,6 @@
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
-
-#include <cstdlib>
 #include <vector>
 
 #include "ln3_internal.h"
@@ -23,11 +21,6 @@ int set_error(int code, const char* fmt, ...) {
 }
 
 void count_launch(int n) { g_launches.fetch_add(static_cast<unsigned long long>(n)); }
-
-bool pdl_enabled() {
-  static const bool on = getenv("LN3_PDL") && atoi(getenv("LN3_PDL")) != 0;  // opt-in: measured no gain inside CUDA graphs
-  return on;
-}
 
 int device_sm_count() {
   static std::atomic<int> sms[64];   // per device ordinal; 0 = not queried yet

@@ -225,8 +225,6 @@ fmha_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
     fence_proxy_async_smem();
   }
   __syncthreads();
-  pdl_launch_dependents();
-  pdl_wait();
 
   if (warp == 8) {
     if (lane == 0) {
@@ -436,8 +434,8 @@ static int fmha_launch(const ln3_fmha_args* a, bool two, cudaStream_t stream) {
   p.o_bs = a->o_bs;
   const int sms = device_sm_count();
   const int grid = p.n_tiles < sms ? static_cast<int>(p.n_tiles) : sms;
-  cudaError_t e = launch_pdl(fmha_fwd_kernel<HD>, dim3(grid), dim3(kThreads), kFmhaSmem<HD>, stream, tq, tk, tv, tk2,
-                             tv2, p, tails);
+  fmha_fwd_kernel<HD><<<grid, kThreads, kFmhaSmem<HD>, stream>>>(tq, tk, tv, tk2, tv2, p, tails);
+  cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error(LN3_ECUDA, "fmha launch: %s", cudaGetErrorString(e));
   count_launch();
   return LN3_OK;

@@ -235,12 +235,6 @@ __device__ __forceinline__ uint64_t make_smem_desc_plain(uint32_t smem_addr, uin
   return d;
 }
 
-// Programmatic dependent launch: the kernel may start while its stream predecessor is still running;
-// pdl_wait() returns once every prerequisite grid has completed and its memory is visible (a no-op for a
-// normal launch), pdl_launch_dependents() lets the NEXT kernel's CTAs be scheduled as ours retire.
-__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-__device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-
 __device__ __forceinline__ int ld_acquire_gpu(const int* p) {
   int v;
   asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");

@@ -17,8 +17,6 @@
 //   patch_embed_triplane  grouped 2x2/s2 conv + the reference's channel interleave -> tokens
 // The decode is < 1 % of the pipeline's FLOPs (20 GFLOP / latent vs 307 TFLOP of sampling), so these
 // kernels favour exact fp32 parity with the reference over tensor-core throughput.
-#include <cstdlib>
-
 #include "common.cuh"
 #include "ln3_internal.h"
 
@@ -222,13 +220,11 @@ conv3x3_tf32_kernel(const ln3_conv_args a) {
 
 // 64 output channels per CTA, or 32 when the 64-channel grid would leave the GPU under two CTAs per SM (the 16 x 16
 // and 32 x 32 levels of the VAE decoder: 192 CTAs; the kernel is bound by the latency of its staging loads -- ncu
-// long_scoreboard 8.5 cycles per issue, 16 % warps active -- so more, smaller CTAs hide more of it).  LN3_CONV_COT64=1
-// (read once) keeps 64 whenever Cout >= 64.
+// long_scoreboard 8.5 cycles per issue, 16 % warps active -- so more, smaller CTAs hide more of it).
 int conv_cout_tile(int N, int H, int W, int Cout) {
-  static const bool cot_auto = !(getenv("LN3_CONV_COT64") && atoi(getenv("LN3_CONV_COT64")) != 0);
   if (Cout < 64) return 32;
   const long long tiles = static_cast<long long>((H + kCT - 1) / kCT) * ((W + kCT - 1) / kCT);
-  if (cot_auto && tiles * ((Cout + 63) / 64) * N < 2LL * device_sm_count()) return 32;
+  if (tiles * ((Cout + 63) / 64) * N < 2LL * device_sm_count()) return 32;
   return 64;
 }
 

@@ -31,8 +31,6 @@ __device__ __forceinline__ float apply_act(float v, int act) {
 template <int NV>
 __global__ void __launch_bounds__(256)
 norm_modulate_kernel(const ln3_norm_modulate_args a) {
-  pdl_launch_dependents();
-  pdl_wait();
   const int lane = threadIdx.x & 31;
   // grid-stride over rows: the host sizes the grid to one resident wave, so there is no partial last wave
   for (int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); row < a.rows;
@@ -158,7 +156,8 @@ __device__ __forceinline__ bool nm_needs_own_row(const ln3_norm_modulate_args& a
   return a.resid != nullptr && (!nm_outside(a, row) || a.resid_out_gate != nullptr);
 }
 
-// LN3_RESID_L2=1: residual-stream accesses carry the L2 evict_last priority (set once per process)
+// LN3_RESID_L2=1: residual-stream accesses carry the L2 evict_last priority (set once per process).  The branches
+// on it also shape ptxas's register allocation: without them the D = 1024 kernel spills at its 80-register cap.
 __constant__ int c_nm_l2_hint;
 
 // Outputs of the row body: `enabled()` is false for a residual-only pass; `store(row, lane, c, y)` writes the 8
@@ -343,8 +342,6 @@ __device__ __forceinline__ void nm_load_row(const ln3_norm_modulate_args& a, int
 template <int NV8, class Out>
 __global__ void __launch_bounds__(256, 3)
 norm_modulate_wide_kernel(const ln3_norm_modulate_args a, const Out out) {
-  pdl_launch_dependents();
-  pdl_wait();
   const int lane = threadIdx.x & 31;
   // A CTA owns a contiguous run of rows (not a grid-stride comb): consecutive token rows share their sample's
   // shift / scale / gate vectors, which then stay in L1 instead of every SM cycling through all samples' vectors
@@ -421,16 +418,15 @@ static int nm_launch_wide(const ln3_norm_modulate_args* a, const Out& out, cudaS
   const int blocks_needed = (a->rows + kNmWarps - 1) / kNmWarps;
   const int wave3 = device_sm_count() * 3;  // 3 resident blocks per SM at <= 80 registers
   const dim3 grid(blocks_needed < wave3 ? blocks_needed : wave3), block(kNmWarps * 32);
-  cudaError_t le = cudaSuccess;
   switch (a->D / 256) {
-    case 1: le = launch_pdl(norm_modulate_wide_kernel<1, Out>, grid, block, 0, stream, *a, out); break;
-    case 2: le = launch_pdl(norm_modulate_wide_kernel<2, Out>, grid, block, 0, stream, *a, out); break;
-    case 3: le = launch_pdl(norm_modulate_wide_kernel<3, Out>, grid, block, 0, stream, *a, out); break;
-    case 4: le = launch_pdl(norm_modulate_wide_kernel<4, Out>, grid, block, 0, stream, *a, out); break;
-    case 5: le = launch_pdl(norm_modulate_wide_kernel<5, Out>, grid, block, 0, stream, *a, out); break;
-    default: le = launch_pdl(norm_modulate_wide_kernel<6, Out>, grid, block, 0, stream, *a, out); break;
+    case 1: norm_modulate_wide_kernel<1, Out><<<grid, block, 0, stream>>>(*a, out); break;
+    case 2: norm_modulate_wide_kernel<2, Out><<<grid, block, 0, stream>>>(*a, out); break;
+    case 3: norm_modulate_wide_kernel<3, Out><<<grid, block, 0, stream>>>(*a, out); break;
+    case 4: norm_modulate_wide_kernel<4, Out><<<grid, block, 0, stream>>>(*a, out); break;
+    case 5: norm_modulate_wide_kernel<5, Out><<<grid, block, 0, stream>>>(*a, out); break;
+    default: norm_modulate_wide_kernel<6, Out><<<grid, block, 0, stream>>>(*a, out); break;
   }
-  cudaError_t e = le != cudaSuccess ? le : cudaGetLastError();
+  cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error(LN3_ECUDA, "norm_modulate launch: %s", cudaGetErrorString(e));
   count_launch();
   return LN3_OK;
@@ -442,8 +438,7 @@ int norm_modulate(const ln3_norm_modulate_args* a, cudaStream_t stream) {
   const int blocks_needed = (a->rows + kNmWarps - 1) / kNmWarps;
   const int wave = device_sm_count() * 4;  // 4 x 256-thread blocks resident per SM (<= 64 regs/thread)
   dim3 grid(blocks_needed < wave ? blocks_needed : wave), block(kNmWarps * 32);
-  static const bool wide_enabled = !(getenv("LN3_NORM_WIDE") && atoi(getenv("LN3_NORM_WIDE")) == 0);
-  const bool wide = wide_enabled && a->D % 256 == 0 && a->D <= 1536 && a->ldo % 8 == 0 && nm_wide_input(a) &&
+  const bool wide = a->D % 256 == 0 && a->D <= 1536 && a->ldo % 8 == 0 && nm_wide_input(a) &&
                     (a->out == nullptr || (reinterpret_cast<uintptr_t>(a->out) & 15) == 0);
   if (int rc = nm_l2_hint_once()) return rc;
   if (wide) return nm_launch_wide(a, NmOutBf16{a->out, a->ldo}, stream);

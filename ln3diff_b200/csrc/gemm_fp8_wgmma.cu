@@ -162,8 +162,6 @@ gemm_fp8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
     fence_barrier_init();
   }
   __syncthreads();
-  pdl_launch_dependents();
-  pdl_wait();
 
   // M first inside an N panel: concurrently resident tiles share W panels in the L2 while A panels stream
   if (warp >= 8) {
@@ -250,7 +248,8 @@ int launch(const CUtensorMap& ta, const CUtensorMap& tb, const Fp8Params& p, cud
   const int tiles = ((p.M + BM - 1) / BM) * (p.N / BN);
   const int sms = device_sm_count();
   const int grid = tiles < sms ? tiles : sms;
-  cudaError_t e = launch_pdl(gemm_fp8_kernel<EPI>, dim3(grid), dim3(kThreads), kSmemBytes, stream, ta, tb, p);
+  gemm_fp8_kernel<EPI><<<grid, kThreads, kSmemBytes, stream>>>(ta, tb, p);
+  cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error(LN3_ECUDA, "gemm_fp8 launch: %s", cudaGetErrorString(e));
   count_launch();
   return LN3_OK;

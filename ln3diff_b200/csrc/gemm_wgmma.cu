@@ -19,8 +19,6 @@
 // map, and the fp32 / residual outputs, store straight from the accumulator layout.
 // Each CTA walks tiles blockIdx.x, +gridDim.x, ...; every output element sees the same wgmma instructions in the
 // same k order as with one 64-row warpgroup per tile half, so results do not depend on the schedule.
-#include <cstdlib>
-
 #include "common.cuh"
 #include "ln3_internal.h"
 
@@ -213,8 +211,6 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     fence_barrier_init();
   }
   __syncthreads();
-  pdl_launch_dependents();
-  pdl_wait();  // barrier set-up and descriptor prefetch overlapped the previous kernel
 
   // Tile order: consecutive CTAs walk M first inside an N panel, so the concurrently resident tiles share
   // W panels (L2 reuse) while A panels stream.  With p.n_first they walk N first across the whole width instead:
@@ -336,8 +332,8 @@ static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const CUten
   const int tiles = ((p.M + BM - 1) / BM) * (p.N / BN);
   const int sms = device_sm_count();
   const int grid = tiles < sms ? tiles : sms;
-  cudaError_t e = launch_pdl(gemm_bf16_kernel<ACT, OUT, HN>, dim3(grid), dim3(kGemmThreads), kSmemBytes, stream, ta, tb, to,
-                              p);
+  gemm_bf16_kernel<ACT, OUT, HN><<<grid, kGemmThreads, kSmemBytes, stream>>>(ta, tb, to, p);
+  cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error(LN3_ECUDA, "gemm launch: %s", cudaGetErrorString(e));
   count_launch();
   return LN3_OK;
@@ -419,12 +415,7 @@ int gemm_bf16(const ln3_gemm_args* a, cudaStream_t stream) {
   if (a->out_kind != LN3_OUT_BF16) return set_error(LN3_EINVAL, "gemm: unknown output kind %d", a->out_kind);
   switch (a->act) {
     case LN3_ACT_NONE: return launch_gemm<LN3_ACT_NONE, LN3_OUT_BF16, false>(ta, tb, to, p, stream);
-    case LN3_ACT_GELU_ERF: {
-      // LN3_GELU_EXACT=1: the A&S 7.1.26 form (|error| <= 1.5e-7, 2 MUFU per element) instead of the polynomial
-      static const bool exact = getenv("LN3_GELU_EXACT") && atoi(getenv("LN3_GELU_EXACT")) != 0;
-      if (exact) return launch_gemm<LN3_ACT_GELU_ERF, LN3_OUT_BF16, false>(ta, tb, to, p, stream);
-      return launch_gemm<kActGeluErfPoly, LN3_OUT_BF16, false>(ta, tb, to, p, stream);
-    }
+    case LN3_ACT_GELU_ERF: return launch_gemm<kActGeluErfPoly, LN3_OUT_BF16, false>(ta, tb, to, p, stream);
     case LN3_ACT_GELU_TANH: return launch_gemm<LN3_ACT_GELU_TANH, LN3_OUT_BF16, false>(ta, tb, to, p, stream);
     case LN3_ACT_SILU: return launch_gemm<LN3_ACT_SILU, LN3_OUT_BF16, false>(ta, tb, to, p, stream);
     case LN3_ACT_QUICK_GELU: return launch_gemm<LN3_ACT_QUICK_GELU, LN3_OUT_BF16, false>(ta, tb, to, p, stream);

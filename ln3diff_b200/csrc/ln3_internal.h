@@ -35,27 +35,6 @@ struct DeviceOnce {
   }
 };
 
-// Programmatic dependent launch (opt-in with LN3_PDL=1; 12.05 vs 12.04 ms per forward, i.e. no gain): kernels that call pdl_wait() before their first
-// dependent memory access may be launched with this; their CTAs are scheduled while the previous
-// kernel of the stream drains, hiding launch latency and the per-CTA prologue.
-bool pdl_enabled();
-
-template <typename... KArgs, typename... Args>
-inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,
-                              Args&&... args) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = grid;
-  cfg.blockDim = block;
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = pdl_enabled() ? 1 : 0;
-  return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
-}
-
 // 2-D bf16 tensor map: tensor [rows, cols] with row pitch `ld` elements, box [box_rows, box_cols],
 // 128-byte swizzle (box_cols must be 64), zero fill out of bounds.
 int make_tmap_2d_bf16(CUtensorMap* out, const void* ptr, long long rows, long long cols,

@@ -5,8 +5,6 @@ own native ops, utils/torch_utils/ops/bias_act.cpp:39-60); everything else is th
 """
 from __future__ import annotations
 
-import os
-
 import ctypes as C
 
 import torch
@@ -808,7 +806,7 @@ def _render_image_width(M: int, image_width: int | None) -> int:
     if image_width is None:
         r = int(round(M ** 0.5))
         image_width = r if r * r == M else 0
-    return int(image_width) if os.environ.get("LN3_RENDER_TILES", "1") != "0" else 0
+    return int(image_width)
 
 
 def render_tile_width(M: int, image_width: int | None = None) -> int:
