@@ -430,6 +430,28 @@ int ln3_ode_stage(const ln3_ode_args* args, int stage, void* stream);
 int ln3_ode_initial_step(const ln3_ode_args* args, int phase, void* stream);
 int ln3_ode_step(const ln3_ode_args* args, void* stream);
 
+/* ------------------------------------------------------------------ grouped adaptive Runge-Kutta
+ * The ln3_ode_* arithmetic above for torchdiffeq's other explicit adaptive Runge-Kutta methods (torchdiffeq 0.2.3
+ * bosh3.py, fehlberg2.py, adaptive_heun.py; restated in transport/rk.py), selected by `method`:
+ *   LN3_ODE_DOPRI5         6 stages, order 5, FSAL   (ln3_ode_stage / _initial_step / _step are this method)
+ *   LN3_ODE_BOSH3          3 stages, order 3, FSAL   (Bogacki-Shampine 3(2))
+ *   LN3_ODE_FEHLBERG2      2 stages, order 2         (Runge-Kutta-Fehlberg 2(1))
+ *   LN3_ODE_ADAPTIVE_HEUN  1 stage,  order 2         (Heun-Euler 2(1))
+ * With S = ln3_ode_stages(method): stages 1..S take beta[stage-1] and alpha[stage-1] of the method's tableau; the
+ * step reads k[0 .. S-1]; nfe grows by S per attempt; the controller and the initial step use 1/order in place of
+ * 1/5; the dense output uses the method's mid weights and f1 = k[S-1].  For a tableau that is not FSAL (c_sol is not
+ * the last beta row with a trailing 0), ln3_ode_rk_step first overwrites y_stage with y1 = y + dt sum_j c_sol[j] k_j
+ * (one more launch), and still commits f0 <- k[S-1], the derivative at the last stage's input, as torchdiffeq does.
+ * Everything else, and every rule on the arguments, is that of the dopri5 entry points.  An unknown method returns
+ * LN3_EUNSUPPORTED (ln3_ode_stages returns it too), a stage outside 0..S LN3_EINVAL.
+ */
+enum { LN3_ODE_DOPRI5 = 0, LN3_ODE_BOSH3 = 1, LN3_ODE_FEHLBERG2 = 2, LN3_ODE_ADAPTIVE_HEUN = 3 };
+
+int ln3_ode_stages(int method);
+int ln3_ode_rk_stage(const ln3_ode_args* args, int method, int stage, void* stream);
+int ln3_ode_rk_initial_step(const ln3_ode_args* args, int method, int phase, void* stream);
+int ln3_ode_rk_step(const ln3_ode_args* args, int method, void* stream);
+
 /* ------------------------------------------------------------------ tri-plane volumetric renderer
  * ln3_render_views: the whole of ImportanceRenderer.forward (nsr/volumetric_rendering/renderer.py:
  * 133-307) for the Objaverse presets (nsr/script_util.py:761-797, 838-870): 'auto' ray limits against the

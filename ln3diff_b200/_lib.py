@@ -223,6 +223,8 @@ class OdeArgs(C.Structure):
 
 
 ODE_RUNNING, ODE_DONE, ODE_EMAXSTEPS, ODE_EUNDERFLOW = 0, 1, -1, -2
+# the `method` of the ln3_ode_rk_* entry points (LN3_ODE_DOPRI5 ..), by torchdiffeq method name
+ODE_METHODS = {"dopri5": 0, "bosh3": 1, "fehlberg2": 2, "adaptive_heun": 3}
 
 NORM_NONE, NORM_LAYER, NORM_RMS = 0, 1, 2
 MLP_FP32, MLP_TF32 = 0, 1

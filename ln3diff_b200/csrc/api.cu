@@ -130,7 +130,8 @@ enum { ODE_NEED_STAGE = 1, ODE_NEED_K = 2, ODE_NEED_K0 = 4, ODE_NEED_OUT = 8, OD
 
 static bool misaligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) != 0; }
 
-static int ode_validate(const ln3_ode_args* a, int need, const char* what) {
+// `stages`: the stage derivatives k[0 .. stages-1] that ODE_NEED_K requires.
+static int ode_validate(const ln3_ode_args* a, int need, const char* what, int stages = 6) {
   if (!a) return set_error(LN3_EINVAL, "%s: null args", what);
   if (a->B <= 0 || a->G <= 0) return set_error(LN3_EINVAL, "%s: B and G must be positive", what);
   if (a->n_per_sample <= 0 || a->n_per_sample % 4)
@@ -142,7 +143,7 @@ static int ode_validate(const ln3_ode_args* a, int need, const char* what) {
     return set_error(LN3_EINVAL, "%s: y and f0 must be 16-byte aligned", what);
   if ((need & ODE_NEED_STAGE) && (!a->y_stage || !a->t_rows || misaligned16(a->y_stage)))
     return set_error(LN3_EINVAL, "%s: y_stage (16-byte aligned) and t_rows are required", what);
-  const int nk = (need & ODE_NEED_K) ? 6 : (need & ODE_NEED_K0) ? 1 : 0;
+  const int nk = (need & ODE_NEED_K) ? stages : (need & ODE_NEED_K0) ? 1 : 0;
   for (int j = 0; j < nk; ++j)
     if (!a->k[j] || misaligned16(a->k[j]))
       return set_error(LN3_EINVAL, "%s: k[%d] is null or not 16-byte aligned", what, j);
@@ -381,26 +382,40 @@ size_t ln3_ode_workspace_bytes(int B, long long n_per_sample) {
   if (B <= 0 || n_per_sample <= 0) return 0;
   return ode_workspace_bytes(B, n_per_sample);
 }
-int ln3_ode_stage(const ln3_ode_args* args, int stage, void* stream) {
-  if (stage < 0 || stage > 6) return set_error(LN3_EINVAL, "ode_stage: stage %d is outside 0..6", stage);
+int ln3_ode_stages(int method) { return ode_stages(method); }
+int ln3_ode_rk_stage(const ln3_ode_args* args, int method, int stage, void* stream) {
+  const int S = ode_stages(method);
+  if (S < 0) return S;
+  if (stage < 0 || stage > S) return set_error(LN3_EINVAL, "ode_stage: stage %d is outside 0..%d", stage, S);
   int rc = ode_validate(args, ODE_NEED_STAGE, "ode_stage");
   if (rc != LN3_OK) return rc;
   for (int j = 0; j + 1 < stage; ++j)   // stage i reads k[0 .. i-2]
     if (!args->k[j] || misaligned16(args->k[j]))
       return set_error(LN3_EINVAL, "ode_stage: k[%d] is null or not 16-byte aligned", j);
-  return ode_stage(args, stage, static_cast<cudaStream_t>(stream));
+  return ode_stage(args, method, stage, static_cast<cudaStream_t>(stream));
 }
-int ln3_ode_initial_step(const ln3_ode_args* args, int phase, void* stream) {
+int ln3_ode_rk_initial_step(const ln3_ode_args* args, int method, int phase, void* stream) {
+  const int S = ode_stages(method);
+  if (S < 0) return S;
   if (phase != 0 && phase != 1) return set_error(LN3_EINVAL, "ode_initial_step: phase must be 0 or 1");
   int rc = ode_validate(args, ODE_NEED_WS | (phase == 1 ? ODE_NEED_K0 : 0), "ode_initial_step");
   if (rc != LN3_OK) return rc;
-  return ode_initial_step(args, phase, static_cast<cudaStream_t>(stream));
+  return ode_initial_step(args, method, phase, static_cast<cudaStream_t>(stream));
 }
-int ln3_ode_step(const ln3_ode_args* args, void* stream) {
-  int rc = ode_validate(args, ODE_NEED_STAGE | ODE_NEED_K | ODE_NEED_OUT | ODE_NEED_WS, "ode_step");
+int ln3_ode_rk_step(const ln3_ode_args* args, int method, void* stream) {
+  const int S = ode_stages(method);
+  if (S < 0) return S;
+  int rc = ode_validate(args, ODE_NEED_STAGE | ODE_NEED_K | ODE_NEED_OUT | ODE_NEED_WS, "ode_step", S);
   if (rc != LN3_OK) return rc;
-  return ode_step(args, static_cast<cudaStream_t>(stream));
+  return ode_step(args, method, static_cast<cudaStream_t>(stream));
 }
+int ln3_ode_stage(const ln3_ode_args* args, int stage, void* stream) {
+  return ln3_ode_rk_stage(args, LN3_ODE_DOPRI5, stage, stream);
+}
+int ln3_ode_initial_step(const ln3_ode_args* args, int phase, void* stream) {
+  return ln3_ode_rk_initial_step(args, LN3_ODE_DOPRI5, phase, stream);
+}
+int ln3_ode_step(const ln3_ode_args* args, void* stream) { return ln3_ode_rk_step(args, LN3_ODE_DOPRI5, stream); }
 
 
 size_t ln3_gemm_fp8_workspace_bytes(void) { return gemm_fp8_workspace_bytes(); }

@@ -88,9 +88,10 @@ int patch_embed_triplane(const float* x, const float* w, const float* bias, int 
 int downsample_nhwc(const ln3_conv_args* a, cudaStream_t stream);
 int vae_posterior(const ln3_vae_posterior_args* a, cudaStream_t stream);
 int view_mean_nhwc(const float* x, float* out, int B, int F, int S, int C, cudaStream_t stream);
+int ode_stages(int method);   // stage forwards per attempt, LN3_EUNSUPPORTED for an unknown method
 size_t ode_workspace_bytes(int B, long long n_per_sample);
-int ode_stage(const ln3_ode_args* a, int stage, cudaStream_t stream);
-int ode_initial_step(const ln3_ode_args* a, int phase, cudaStream_t stream);
-int ode_step(const ln3_ode_args* a, cudaStream_t stream);
+int ode_stage(const ln3_ode_args* a, int method, int stage, cudaStream_t stream);
+int ode_initial_step(const ln3_ode_args* a, int method, int phase, cudaStream_t stream);
+int ode_step(const ln3_ode_args* a, int method, cudaStream_t stream);
 
 }  // namespace ln3

@@ -1,9 +1,11 @@
-// Grouped adaptive Dormand-Prince 5(4): the per-attempt arithmetic of transport/dopri5.py:odeint_dopri5 for G
-// independent groups of rows in one batch, with the accept / reject control on the device.
-//   ode_stage    y_stage = y + dt_g sum_j beta_ij k_j and the per-row fp32 forward time (one launch per stage)
+// Grouped adaptive explicit Runge-Kutta: the per-attempt arithmetic of transport/rk.py:odeint_rk_adaptive (dopri5,
+// bosh3, fehlberg2, adaptive_heun) for G independent groups of rows in one batch, with the accept / reject control on
+// the device.  Each kernel takes the method and reads its Butcher tableau from c_tab.
+//   ode_stage    y_stage = y + dt_g sum_j beta_ij k_j and the per-row fp32 forward time (one launch per stage); for
+//                a tableau that is not FSAL, the solution y1 = y + dt_g sum_j c_sol_j k_j after the last stage
 //   ode_norm     fixed-partition float64 partial sums of squared scaled quantities, per (row, 1024-element chunk)
 //   ode_control  one CTA per group: its rows' partials in row, chunk order -> ratio / step controller / counters
-//   ode_commit   y <- y1, f0 <- f1 on accept (FSAL), the dense output at t_end when the group finishes
+//   ode_commit   y <- y1, f0 <- f1 = k[last] on accept, the dense output at t_end when the group finishes
 // Every fp32 operation that the host solver performs on tensors is individually rounded here in the same order (no
 // FMA contraction), and every float64 scalar operation likewise, so the only intended difference from the host
 // solver is the order of the error-norm reduction.  Reference call sites are cited in include/ln3b200.h.
@@ -18,22 +20,56 @@ namespace {
 
 constexpr int kThreads = 256;
 constexpr int kChunk = kThreads * 4;   // elements per partial sum: one float4 per thread
+constexpr int kMethods = 4;            // LN3_ODE_DOPRI5 .. LN3_ODE_ADAPTIVE_HEUN
 
-// transport/dopri5.py _ALPHA, _BETA, _C_ERROR, _C_MID (the same double expressions)
-__constant__ double c_alpha[6] = {1.0 / 5, 3.0 / 10, 4.0 / 5, 8.0 / 9, 1.0, 1.0};
-__constant__ double c_beta[6][6] = {
-    {1.0 / 5, 0, 0, 0, 0, 0},
-    {3.0 / 40, 9.0 / 40, 0, 0, 0, 0},
-    {44.0 / 45, -56.0 / 15, 32.0 / 9, 0, 0, 0},
-    {19372.0 / 6561, -25360.0 / 2187, 64448.0 / 6561, -212.0 / 729, 0, 0},
-    {9017.0 / 3168, -355.0 / 33, 46732.0 / 5247, 49.0 / 176, -5103.0 / 18656, 0},
-    {35.0 / 384, 0.0, 500.0 / 1113, 125.0 / 192, -2187.0 / 6784, 11.0 / 84}};
-__constant__ double c_err[7] = {35.0 / 384 - 1951.0 / 21600, 0.0, 500.0 / 1113 - 22642.0 / 50085,
-                                125.0 / 192 - 451.0 / 720, -2187.0 / 6784 - -12231.0 / 42400,
-                                11.0 / 84 - 649.0 / 6300, -1.0 / 60.0};
-__constant__ double c_mid[7] = {6025192743.0 / 30085553152.0 / 2, 0.0, 51252292925.0 / 65400821598.0 / 2,
-                                -2691868925.0 / 45128329728.0 / 2, 187940372067.0 / 1594534317056.0 / 2,
-                                -1776094331.0 / 19743644256.0 / 2, 11237099.0 / 235043384.0 / 2};
+// transport/rk.py TABLEAUS (the same double expressions).  beta rows, c_sol, c_err and c_mid are zero-padded to
+// 7 terms (k_0 = f0 .. k_6); a zero coefficient is skipped, as _lincomb skips it.
+struct Tableau {
+  int stages;        // stage forwards per attempt (beta rows)
+  int fsal;          // c_sol is the last beta row with a trailing 0: y1 is the last stage's input
+  double expo;       // 1 / order: the step controller's and the initial step's exponent
+  double alpha[6];
+  double beta[6][7];
+  double c_sol[7];
+  double c_err[7];
+  double c_mid[7];
+};
+
+constexpr Tableau kTab[kMethods] = {
+    {6, 1, 1.0 / 5,   // dopri5
+     {1.0 / 5, 3.0 / 10, 4.0 / 5, 8.0 / 9, 1.0, 1.0},
+     {{1.0 / 5},
+      {3.0 / 40, 9.0 / 40},
+      {44.0 / 45, -56.0 / 15, 32.0 / 9},
+      {19372.0 / 6561, -25360.0 / 2187, 64448.0 / 6561, -212.0 / 729},
+      {9017.0 / 3168, -355.0 / 33, 46732.0 / 5247, 49.0 / 176, -5103.0 / 18656},
+      {35.0 / 384, 0.0, 500.0 / 1113, 125.0 / 192, -2187.0 / 6784, 11.0 / 84}},
+     {35.0 / 384, 0.0, 500.0 / 1113, 125.0 / 192, -2187.0 / 6784, 11.0 / 84, 0.0},
+     {35.0 / 384 - 1951.0 / 21600, 0.0, 500.0 / 1113 - 22642.0 / 50085, 125.0 / 192 - 451.0 / 720,
+      -2187.0 / 6784 - -12231.0 / 42400, 11.0 / 84 - 649.0 / 6300, -1.0 / 60.0},
+     {6025192743.0 / 30085553152.0 / 2, 0.0, 51252292925.0 / 65400821598.0 / 2,
+      -2691868925.0 / 45128329728.0 / 2, 187940372067.0 / 1594534317056.0 / 2,
+      -1776094331.0 / 19743644256.0 / 2, 11237099.0 / 235043384.0 / 2}},
+    {3, 1, 1.0 / 3,   // bosh3 (Bogacki-Shampine 3(2))
+     {1.0 / 2, 3.0 / 4, 1.0},
+     {{1.0 / 2}, {0.0, 3.0 / 4}, {2.0 / 9, 1.0 / 3, 4.0 / 9}},
+     {2.0 / 9, 1.0 / 3, 4.0 / 9, 0.0},
+     {2.0 / 9 - 7.0 / 24, 1.0 / 3 - 1.0 / 4, 4.0 / 9 - 1.0 / 3, -1.0 / 8},
+     {0.0, 0.5, 0.0, 0.0}},
+    {2, 0, 1.0 / 2,   // fehlberg2 (Runge-Kutta-Fehlberg 2(1))
+     {1.0 / 2, 1.0},
+     {{1.0 / 2}, {1.0 / 256, 255.0 / 256}},
+     {1.0 / 512, 255.0 / 256, 1.0 / 512},
+     {-1.0 / 512, 0.0, 1.0 / 512},
+     {0.0, 0.5, 0.0}},
+    {1, 0, 1.0 / 2,   // adaptive_heun (Heun-Euler 2(1))
+     {1.0},
+     {{1.0}},
+     {0.5, 0.5},
+     {0.5, -0.5},
+     {0.5, 0.0}},
+};
+__constant__ Tableau c_tab[kMethods] = {kTab[0], kTab[1], kTab[2], kTab[3]};
 
 enum { MODE_ERR = 0, MODE_INIT0 = 1, MODE_INIT1 = 2 };
 
@@ -56,7 +92,9 @@ __device__ __forceinline__ void st4(float* p, long long off, const float v[4]) {
 __device__ __forceinline__ const float* kptr(const ln3_ode_args& a, int j) { return j == 0 ? a.f0 : a.k[j - 1]; }
 
 // ------------------------------------------------------------------ stage combination
-__global__ void __launch_bounds__(kThreads) ode_stage_kernel(const ln3_ode_args a, int stage) {
+// stage 1..stages: the stage inputs; stage == stages + 1 (tableaus that are not FSAL): y1 = y + dt sum_j c_sol_j k_j
+// into y_stage, no forward time.
+__global__ void __launch_bounds__(kThreads) ode_stage_kernel(const ln3_ode_args a, int method, int stage) {
   const int r = blockIdx.y;
   const ln3_ode_group* s = a.state + a.row_group[r];
   if (s->status != LN3_ODE_RUNNING) return;
@@ -76,17 +114,20 @@ __global__ void __launch_bounds__(kThreads) ode_stage_kernel(const ln3_ode_args 
     }
     return;
   }
+  const Tableau& tb = c_tab[method];
   const int row = stage - 1;
-  if (blockIdx.x == 0 && threadIdx.x == 0)
-    a.t_rows[r] = static_cast<float>(__dadd_rn(t, __dmul_rn(c_alpha[row], dt)));
-  float cf[6];
+  const bool sol = row == tb.stages;
+  const double* coef = sol ? tb.c_sol : tb.beta[row];
+  if (!sol && blockIdx.x == 0 && threadIdx.x == 0)
+    a.t_rows[r] = static_cast<float>(__dadd_rn(t, __dmul_rn(tb.alpha[row], dt)));
+  float cf[7];
 #pragma unroll
-  for (int j = 0; j < 6; ++j) cf[j] = static_cast<float>(__dmul_rn(c_beta[row][j], dt));
+  for (int j = 0; j < 7; ++j) cf[j] = static_cast<float>(__dmul_rn(coef[j], dt));
   for (long long i = blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += static_cast<long long>(gridDim.x) * blockDim.x) {
     float acc[4], k[4];
     ld4(a.y, base + i * 4, acc);
     for (int j = 0; j < stage; ++j) {
-      if (c_beta[row][j] == 0.0) continue;   // _lincomb skips zero coefficients
+      if (coef[j] == 0.0) continue;   // _lincomb skips zero coefficients
       ld4(kptr(a, j), base + i * 4, k);
 #pragma unroll
       for (int e = 0; e < 4; ++e) acc[e] = add(acc[e], mul(k[e], cf[j]));
@@ -115,7 +156,7 @@ __device__ __forceinline__ double block_sum_d(double v, double* sh) {
 }
 
 // grid (nchunk, B): partial[(r * nchunk + c) * 2 + q] = sum over chunk c of row r of q-th squared quantity
-__global__ void __launch_bounds__(kThreads) ode_norm_kernel(const ln3_ode_args a, int mode) {
+__global__ void __launch_bounds__(kThreads) ode_norm_kernel(const ln3_ode_args a, int method, int mode) {
   __shared__ double sh[kThreads / 32];
   const int r = blockIdx.y, c = blockIdx.x;
   if (a.state[a.row_group[r]].status != LN3_ODE_RUNNING) return;
@@ -130,6 +171,7 @@ __global__ void __launch_bounds__(kThreads) ode_norm_kernel(const ln3_ode_args a
     if (mode == MODE_ERR) {
       const double dt = a.state[a.row_group[r]].dt;
       float err[4] = {0.f, 0.f, 0.f, 0.f}, k[4], y1[4];
+      const double* c_err = c_tab[method].c_err;
       for (int j = 0; j < 7; ++j) {
         if (c_err[j] == 0.0) continue;
         const float cj = static_cast<float>(__dmul_rn(c_err[j], dt));
@@ -178,7 +220,7 @@ __device__ __forceinline__ void check_next_attempt(ln3_ode_group& s, int max_num
 }
 
 // grid G: group g's sums over its rows (ascending) and their chunks (ascending), then the scalar control logic.
-__global__ void __launch_bounds__(kThreads) ode_control_kernel(const ln3_ode_args a, int mode, int nchunk) {
+__global__ void __launch_bounds__(kThreads) ode_control_kernel(const ln3_ode_args a, int method, int mode, int nchunk) {
   __shared__ double sh[kThreads / 32];
   const int g = blockIdx.x;
   ln3_ode_group* sp = a.state + g;
@@ -212,7 +254,7 @@ __global__ void __launch_bounds__(kThreads) ode_control_kernel(const ln3_ode_arg
     const double d2 = sqrt(s0 / count) / h0;
     double h1;
     if (d1 <= 1e-15 && d2 <= 1e-15) h1 = py_max(1e-6, h0 * 1e-3);
-    else h1 = pow(0.01 / py_max(d1, d2), 1.0 / 5.0);
+    else h1 = pow(0.01 / py_max(d1, d2), c_tab[method].expo);
     s.dt = py_min(100 * h0, h1);
     s.nfe = 2;
     s.event = 0;
@@ -221,7 +263,7 @@ __global__ void __launch_bounds__(kThreads) ode_control_kernel(const ln3_ode_arg
     const double ratio = sqrt(s0 / count), dt = s.dt;
     s.ratio = ratio;
     s.dt_step = dt;
-    s.nfe += 6;
+    s.nfe += c_tab[method].stages;
     if (ratio <= 1.0) {
       s.t_prev = s.t;
       s.t = __dadd_rn(s.t, dt);
@@ -236,7 +278,7 @@ __global__ void __launch_bounds__(kThreads) ode_control_kernel(const ln3_ode_arg
       s.dt = dt * a.ifactor;
     } else {
       const double df = ratio < 1.0 ? 1.0 : a.dfactor;
-      s.dt = dt * py_min(a.ifactor, py_max(a.safety / pow(ratio, 0.2), df));
+      s.dt = dt * py_min(a.ifactor, py_max(a.safety / pow(ratio, c_tab[method].expo), df));
     }
     if (s.status == LN3_ODE_RUNNING) check_next_attempt(s, a.max_num_steps);
   }
@@ -244,7 +286,7 @@ __global__ void __launch_bounds__(kThreads) ode_control_kernel(const ln3_ode_arg
 }
 
 // ------------------------------------------------------------------ commit + dense output
-__global__ void __launch_bounds__(kThreads) ode_commit_kernel(const ln3_ode_args a) {
+__global__ void __launch_bounds__(kThreads) ode_commit_kernel(const ln3_ode_args a, int method) {
   const int r = blockIdx.y;
   const ln3_ode_group* sp = a.state + a.row_group[r];
   const int ev = sp->event;
@@ -252,12 +294,13 @@ __global__ void __launch_bounds__(kThreads) ode_commit_kernel(const ln3_ode_args
   const double dt = sp->dt_step;
   const long long base = static_cast<long long>(r) * a.n_per_sample;
   const long long n4 = a.n_per_sample >> 2;
-  const float* f1p = a.k[5];
+  const Tableau& tb = c_tab[method];
+  const float* f1p = a.k[tb.stages - 1];   // f1 = k[last], also when y1 was recomputed from c_sol
   float cm[7];
   float fdt = 0.f, f2dt = 0.f, x1 = 0.f, x2 = 0.f, x3 = 0.f, x4 = 0.f;
   if (ev == 2) {
 #pragma unroll
-    for (int j = 0; j < 7; ++j) cm[j] = static_cast<float>(__dmul_rn(c_mid[j], dt));
+    for (int j = 0; j < 7; ++j) cm[j] = static_cast<float>(__dmul_rn(tb.c_mid[j], dt));
     fdt = static_cast<float>(dt);
     f2dt = static_cast<float>(2 * dt);
     const double x = (a.t_end - sp->t_prev) / (sp->t - sp->t_prev);   // _interp_eval
@@ -276,7 +319,7 @@ __global__ void __launch_bounds__(kThreads) ode_commit_kernel(const ln3_ode_args
 #pragma unroll
       for (int e = 0; e < 4; ++e) ym[e] = y[e];
       for (int j = 0; j < 7; ++j) {
-        if (c_mid[j] == 0.0) continue;
+        if (tb.c_mid[j] == 0.0) continue;
         ld4(kptr(a, j), off, k);
 #pragma unroll
         for (int e = 0; e < 4; ++e) ym[e] = add(ym[e], mul(k[e], cm[j]));
@@ -319,34 +362,43 @@ dim3 row_grid(const ln3_ode_args* a) {
   return dim3(static_cast<unsigned>(gx), a->B);
 }
 
-int launch_norm_control(const ln3_ode_args* a, int mode, cudaStream_t stream) {
+int launch_norm_control(const ln3_ode_args* a, int method, int mode, cudaStream_t stream) {
   const long long nc = nchunks(a->n_per_sample);
   if (nc > 0x7fffffffLL) return set_error(LN3_EUNSUPPORTED, "ode: n_per_sample too large");
-  ode_norm_kernel<<<dim3(static_cast<unsigned>(nc), a->B), kThreads, 0, stream>>>(*a, mode);
-  ode_control_kernel<<<a->G, kThreads, 0, stream>>>(*a, mode, static_cast<int>(nc));
+  ode_norm_kernel<<<dim3(static_cast<unsigned>(nc), a->B), kThreads, 0, stream>>>(*a, method, mode);
+  ode_control_kernel<<<a->G, kThreads, 0, stream>>>(*a, method, mode, static_cast<int>(nc));
   return launched("ode_norm/control", 2);
 }
 
 }  // namespace
 
-// Arguments are validated by the ln3_ode_* entry points (api.cu).
+// Arguments are validated by the ln3_ode_* entry points (api.cu), the method by ode_stages.
+int ode_stages(int method) {
+  if (method < 0 || method >= kMethods) return set_error(LN3_EUNSUPPORTED, "ode: unknown method %d", method);
+  return kTab[method].stages;
+}
+
 size_t ode_workspace_bytes(int B, long long n_per_sample) {
   return static_cast<size_t>(B) * static_cast<size_t>(nchunks(n_per_sample)) * 2 * sizeof(double);
 }
 
-int ode_stage(const ln3_ode_args* a, int stage, cudaStream_t stream) {
-  ode_stage_kernel<<<row_grid(a), kThreads, 0, stream>>>(*a, stage);
+int ode_stage(const ln3_ode_args* a, int method, int stage, cudaStream_t stream) {
+  ode_stage_kernel<<<row_grid(a), kThreads, 0, stream>>>(*a, method, stage);
   return launched("ode_stage", 1);
 }
 
-int ode_initial_step(const ln3_ode_args* a, int phase, cudaStream_t stream) {
-  return launch_norm_control(a, phase == 0 ? MODE_INIT0 : MODE_INIT1, stream);
+int ode_initial_step(const ln3_ode_args* a, int method, int phase, cudaStream_t stream) {
+  return launch_norm_control(a, method, phase == 0 ? MODE_INIT0 : MODE_INIT1, stream);
 }
 
-int ode_step(const ln3_ode_args* a, cudaStream_t stream) {
-  const int rc = launch_norm_control(a, MODE_ERR, stream);
+int ode_step(const ln3_ode_args* a, int method, cudaStream_t stream) {
+  if (!kTab[method].fsal) {   // y_stage <- y1 = y + dt c_sol . k; f1 stays k[last] (torchdiffeq's _runge_kutta_step)
+    const int rc = ode_stage(a, method, kTab[method].stages + 1, stream);
+    if (rc != LN3_OK) return rc;
+  }
+  const int rc = launch_norm_control(a, method, MODE_ERR, stream);
   if (rc != LN3_OK) return rc;
-  ode_commit_kernel<<<row_grid(a), kThreads, 0, stream>>>(*a);
+  ode_commit_kernel<<<row_grid(a), kThreads, 0, stream>>>(*a, method);
   return launched("ode_commit", 1);
 }
 

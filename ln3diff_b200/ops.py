@@ -657,26 +657,37 @@ def _ode_k(a: _lib.OdeArgs, ks) -> None:
     a.ks = tuple(ks)                                  # keeps the stage tensors alive with the argument block
 
 
-def ode_stage(a: _lib.OdeArgs, stage: int, ks=()) -> None:
-    """ln3_ode_stage: y_stage and t_rows of DP stage `stage` (1..6, reading f0 and ks[:stage-1]) or of the
-    initial-step probe (stage 0)."""
+def ode_stages(method: int = _lib.ODE_METHODS["dopri5"]) -> int:
+    """ln3_ode_stages: the stage forwards per attempt of an ln3_ode_rk_* method (_lib.ODE_METHODS)."""
+    n = int(_lib.lib().ln3_ode_stages(int(method)))
+    if n < 0:
+        _lib.check(n, "ln3_ode_stages")
+    return n
+
+
+def ode_stage(a: _lib.OdeArgs, stage: int, ks=(), method: int = _lib.ODE_METHODS["dopri5"]) -> None:
+    """ln3_ode_rk_stage: y_stage and t_rows of stage `stage` (1..S of `method`, reading f0 and ks[:stage-1]) or of
+    the initial-step probe (stage 0)."""
     _req(0 <= stage <= 6 and len(ks) >= max(stage - 1, 0), "stage i needs the i-1 previous stage derivatives")
     _ode_k(a, ks)
-    _lib.check(_lib.lib().ln3_ode_stage(C.byref(a), stage, _lib.current_stream()), "ln3_ode_stage")
+    _lib.check(_lib.lib().ln3_ode_rk_stage(C.byref(a), int(method), stage, _lib.current_stream()), "ln3_ode_stage")
 
 
-def ode_initial_step(a: _lib.OdeArgs, phase: int, k0: torch.Tensor | None = None) -> None:
-    """ln3_ode_initial_step: phase 0 -> h0 per group; phase 1 (k0 = forward at the stage-0 probe) -> first dt."""
+def ode_initial_step(a: _lib.OdeArgs, phase: int, k0: torch.Tensor | None = None,
+                     method: int = _lib.ODE_METHODS["dopri5"]) -> None:
+    """ln3_ode_rk_initial_step: phase 0 -> h0 per group; phase 1 (k0 = forward at the stage-0 probe) -> first dt."""
     _req(phase in (0, 1) and (phase == 0 or k0 is not None), "phase 1 needs k0")
     _ode_k(a, () if k0 is None else (k0,))
-    _lib.check(_lib.lib().ln3_ode_initial_step(C.byref(a), phase, _lib.current_stream()), "ln3_ode_initial_step")
+    _lib.check(_lib.lib().ln3_ode_rk_initial_step(C.byref(a), int(method), phase, _lib.current_stream()),
+               "ln3_ode_initial_step")
 
 
-def ode_step(a: _lib.OdeArgs, ks) -> None:
-    """ln3_ode_step: error ratio, accept / reject, next dt, commit and dense output, from the six stage derivatives."""
-    _req(len(ks) == 6, "ode_step needs the six stage derivatives")
+def ode_step(a: _lib.OdeArgs, ks, method: int = _lib.ODE_METHODS["dopri5"]) -> None:
+    """ln3_ode_rk_step: error ratio, accept / reject, next dt, commit and dense output, from the S stage
+    derivatives of `method` (six for dopri5)."""
+    _req(len(ks) == ode_stages(method), "ode_step needs one stage derivative per stage of the method")
     _ode_k(a, ks)
-    _lib.check(_lib.lib().ln3_ode_step(C.byref(a), _lib.current_stream()), "ln3_ode_step")
+    _lib.check(_lib.lib().ln3_ode_rk_step(C.byref(a), int(method), _lib.current_stream()), "ln3_ode_step")
 
 
 def generate_rays(cams: torch.Tensor, res: int):

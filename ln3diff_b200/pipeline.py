@@ -450,21 +450,28 @@ def flow_batch_context(c: dict, uc: dict, dev=None, dtype=torch.float32) -> dict
 
 @torch.no_grad()
 def sample_flow_batched(model, c: dict, uc: dict, num_samples: int, seed: int = 42, num_steps: int = 250,
-                        cfg_scale: float = 4.0, dtype=torch.float32, sde: dict | None = None):
-    """`sample_flow` with its default dopri5 solver for P conditions in one denoiser batch.  c / uc hold P conditions
-    stacked condition-major, each repeated `num_samples` times as `condition_prompt` returns it ((P*N, ...) per key).
-    The batch is cat([zs, zs]) of 2PN rows with context cat((c, uc)); every condition runs its own adaptive dopri5
-    trajectory (transport/dopri5.py:odeint_dopri5_grouped), so its latents do not depend on the other conditions in
-    the batch.  The noise is `flow_batch_noise` (sample_flow's draw for every condition).  num_steps is the output
-    grid of sample_ode; dopri5 only uses its last point, t = 1.
-    Returns (latents (P, N, 12, 32, 32) fp32, stats) with per-condition lists nfe / accepted / rejected and the
-    batch's forward count batch_nfe.
+                        cfg_scale: float = 4.0, dtype=torch.float32, sde: dict | None = None,
+                        sampling_method: str = "dopri5"):
+    """`sample_flow` for P conditions in one denoiser batch.  c / uc hold P conditions stacked condition-major, each
+    repeated `num_samples` times as `condition_prompt` returns it ((P*N, ...) per key).  The batch is cat([zs, zs])
+    of 2PN rows with context cat((c, uc)); the noise is `flow_batch_noise` (sample_flow's draw for every condition).
+    num_steps is the output grid of sample_ode.
+
+    `sampling_method`: an adaptive method (dopri5, bosh3, fehlberg2, adaptive_heun) runs every condition on its own
+    trajectory (transport/rk.py:odeint_rk_adaptive_grouped), so its latents do not depend on the other conditions in
+    the batch; it only uses the grid's last point, t = 1.  A fixed-grid method (euler, midpoint, heun, rk4) steps the
+    whole batch on the grid, which every condition shares.  Any other name raises NotImplementedError.
+    Returns (latents (P, N, 12, 32, 32) fp32, stats) with per-condition lists nfe (and, for an adaptive method,
+    accepted / rejected) and the batch's forward count batch_nfe.
 
     With `sde` (a dict of `sample_sde` keywords, see `sample_flow_sde`) the P conditions instead run the SDE on the
     shared fixed grid of num_steps points; every condition reads the noise draw its own `sample_flow(..., sde=)` call
     would make, so its latents are that call's up to the rounding of the batched GEMMs.  stats then hold nfe (per
     condition) and batch_nfe, both the forward count."""
-    from .transport.dopri5 import odeint_dopri5_grouped
+    from .transport import rk
+    _check_sde_method(sde, sampling_method)
+    if sampling_method not in rk.FIXED_GRID_METHODS:
+        rk.tableau(sampling_method)                   # NotImplementedError naming the built methods
     dev = next(model.parameters()).device
     if dev.type != "cuda":
         raise RuntimeError("sample_flow_batched runs on CUDA only (no CPU fallback)")
@@ -479,16 +486,29 @@ def sample_flow_batched(model, c: dict, uc: dict, num_samples: int, seed: int = 
     if sde is not None:
         x, plan = sample_flow_sde(model, zs, ctx, N, num_steps, cfg_scale, sde)
         return x[:P * N].reshape(P, N, *shape), dict(nfe=[plan["forwards"]] * P, batch_nfe=plan["forwards"])
-    grid = torch.linspace(0, 1, num_steps)            # sample_ode's grid: dopri5 integrates to its last point
+    if sampling_method in rk.FIXED_GRID_METHODS:
+        from .transport import Sampler, create_transport
+        fn = Sampler(create_transport(snr_type="lognorm")).sample_ode(sampling_method=sampling_method,
+                                                                       num_steps=num_steps)
+        y = fn(torch.cat([zs, zs], 0), model.forward_with_cfg, context=ctx, cfg_scale=cfg_scale)[-1]
+        nfe = rk.FIXED_GRID_FORWARDS[sampling_method] * (num_steps - 1)
+        return y[:P * N].reshape(P, N, *shape), dict(nfe=[nfe] * P, batch_nfe=nfe)
+    grid = torch.linspace(0, 1, num_steps)            # sample_ode's grid: the solver integrates to its last point
     fn = lambda t, x: model.forward_with_cfg(x, t, ctx, cfg_scale)
-    y, stats = odeint_dopri5_grouped(fn, torch.cat([zs, zs], 0), flow_batch_row_groups(P, N), P,
-                                     t0=float(grid[0]), t1=float(grid[-1]), rtol=1e-3, atol=1e-6)
+    if sampling_method == "dopri5":
+        from .transport.dopri5 import odeint_dopri5_grouped
+        y, stats = odeint_dopri5_grouped(fn, torch.cat([zs, zs], 0), flow_batch_row_groups(P, N), P,
+                                         t0=float(grid[0]), t1=float(grid[-1]), rtol=1e-3, atol=1e-6)
+    else:
+        y, stats = rk.odeint_rk_adaptive_grouped(fn, torch.cat([zs, zs], 0), flow_batch_row_groups(P, N), P,
+                                                 t0=float(grid[0]), t1=float(grid[-1]), method=sampling_method,
+                                                 rtol=1e-3, atol=1e-6)
     return y[:P * N].reshape(P, N, *shape), stats
 
 
 @torch.no_grad()
 def _conds_to_3d(conditioner, model, decoder, cond_key, prompts, cameras, num_samples, seed, num_steps, cfg_scale,
-                 resolution, dtype, sde):
+                 resolution, dtype, sde, sampling_method):
     """`_cond_to_3d` for a list of conditions: the conditioner once per condition, in order, one batched sample,
     then decode and render of every latent.  The render noise is one device draw for the batch."""
     dev = next(model.parameters()).device
@@ -496,7 +516,7 @@ def _conds_to_3d(conditioner, model, decoder, cond_key, prompts, cameras, num_sa
     c = {k: torch.cat([ci[k] for ci in cs]) if isinstance(cs[0][k], torch.Tensor) else cs[0][k] for k in cs[0]}
     uc = {k: torch.cat([ui[k] for ui in ucs]) if isinstance(ucs[0][k], torch.Tensor) else ucs[0][k] for k in ucs[0]}
     latents, stats = sample_flow_batched(model, c, uc, num_samples, seed=seed, num_steps=num_steps,
-                                         cfg_scale=cfg_scale, dtype=dtype, sde=sde)
+                                         cfg_scale=cfg_scale, dtype=dtype, sde=sde, sampling_method=sampling_method)
     P, N = latents.shape[:2]
     out = decode_and_render(decoder, latents.reshape(P * N, *latents.shape[2:]), cameras[:24].to(dev), resolution)
     return latents, {k: v.reshape(P, N, *v.shape[1:]) for k, v in out.items()}, stats
@@ -505,31 +525,33 @@ def _conds_to_3d(conditioner, model, decoder, cond_key, prompts, cameras, num_sa
 @torch.no_grad()
 def images_to_3d(conditioner, model, decoder, images: torch.Tensor, cameras: torch.Tensor, num_samples: int = 4,
                  seed: int = 42, num_steps: int = 250, cfg_scale: float = 4.0, resolution: int = 192,
-                 dtype=torch.float32, sde: dict | None = None):
-    """`image_to_3d` with dopri5 for P images (P, 3, H, W) in [-1, 1] in one denoiser batch.  Each image's latents
-    are those `image_to_3d` gives for it alone up to the rounding of the batched GEMMs; the renders use one device
-    noise draw for the whole batch, so they are not bit-identical to sequential calls.  `sde`: see sample_flow_batched.
+                 dtype=torch.float32, sde: dict | None = None, sampling_method: str = "dopri5"):
+    """`image_to_3d` for P images (P, 3, H, W) in [-1, 1] in one denoiser batch.  Each image's latents are those
+    `image_to_3d` gives for it alone up to the rounding of the batched GEMMs; the renders use one device noise draw
+    for the whole batch, so they are not bit-identical to sequential calls.  `sde`, `sampling_method`: see
+    sample_flow_batched.
     Returns (latents (P, N, 12, 32, 32), render dict with (P, N, 24, ...) tensors, per-image stats)."""
     dev = next(model.parameters()).device
     imgs = [images[i:i + 1].to(dev).to(dtype).clone() for i in range(images.shape[0])]   # own, aligned buffers
     return _conds_to_3d(conditioner, model, decoder, "img", imgs, cameras, num_samples, seed, num_steps, cfg_scale,
-                        resolution, dtype, sde)
+                        resolution, dtype, sde, sampling_method)
 
 
 @torch.no_grad()
 def mvs_to_3d(conditioner, model, decoder, mv_images: torch.Tensor, mv_cameras: torch.Tensor, cameras: torch.Tensor,
               num_samples: int = 4, seed: int = 42, num_steps: int = 250, cfg_scale: float = 4.0,
-              resolution: int = 192, dtype=torch.float32, sde: dict | None = None):
-    """`mv_to_3d` with dopri5 for P multi-view conditions, mv_images (P, V, 3, H, W) and mv_cameras (P, V, 25), in one
+              resolution: int = 192, dtype=torch.float32, sde: dict | None = None, sampling_method: str = "dopri5"):
+    """`mv_to_3d` for P multi-view conditions, mv_images (P, V, 3, H, W) and mv_cameras (P, V, 25), in one
     denoiser batch.  The conditioner runs once per condition in order, so its `aug_c` camera draws follow the same
     sequence as P sequential `mv_to_3d` calls.  Every condition gets its own copy of its views and cameras (the
     conditioner's kernels want 16-byte aligned rows), so with `aug_c=True` the rotations apply to those copies and the
-    caller's `mv_cameras` is left as it is.  `sde`: see sample_flow_batched.  Returns as `images_to_3d`."""
+    caller's `mv_cameras` is left as it is.  `sde`, `sampling_method`: see sample_flow_batched.  Returns as
+    `images_to_3d`."""
     dev = next(model.parameters()).device
     own = lambda x, i: x[i:i + 1].to(dev).to(dtype).clone()
     prompts = [{"img": own(mv_images, i), "c": own(mv_cameras, i)} for i in range(mv_images.shape[0])]
     return _conds_to_3d(conditioner, model, decoder, "img-c", prompts, cameras, num_samples, seed, num_steps,
-                        cfg_scale, resolution, dtype, sde)
+                        cfg_scale, resolution, dtype, sde, sampling_method)
 
 
 @torch.no_grad()

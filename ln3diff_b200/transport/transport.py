@@ -130,6 +130,8 @@ class ode:
                     y = self._axpy(self._axpy(y, half, k1, ch), half, k2, ch)
                 ys.append(y)
             return th.stack(ys, 0)
+        if self.sampler_type == "rk4":
+            return self._rk4(x, _fn, B, device)
         try:
             from torchdiffeq import odeint  # the reference's own third-party solver, when it is installed
         except ImportError:
@@ -141,9 +143,44 @@ class ode:
             from .dopri5 import odeint_dopri5
             self.last_stats = {}
             return odeint_dopri5(_fn, x, t, rtol=self.rtol, atol=self.atol, stats=self.last_stats)
-        raise NotImplementedError(
-            f"sampling_method='{self.sampler_type}' needs torchdiffeq (un-vendored dependency of the reference); "
-            "'dopri5' and the fixed-grid 'euler' / 'heun' / 'midpoint' solvers are built in")
+        from .rk import odeint_rk_adaptive, tableau
+        tableau(self.sampler_type)     # NotImplementedError naming the built methods for any other name
+        self.last_stats = {}           # bosh3 / fehlberg2 / adaptive_heun: restated solvers, see transport/rk.py
+        return odeint_rk_adaptive(_fn, x, t, self.sampler_type, rtol=self.rtol, atol=self.atol,
+                                  stats=self.last_stats)
+
+    def _rk4(self, x, _fn, B, device):
+        """torchdiffeq's fixed-grid rk4 (rk4_alt_step_func, the 3/8 rule) on the output grid.  CUDA fp32 states take
+        each stage input and the update through ln3_sampler_affine_update (five launches per step, coefficients
+        uploaded once); any other state runs transport/rk.py:odeint_rk4's tensor arithmetic."""
+        from .rk import _ONE_THIRD, _TWO_THIRDS, odeint_rk4
+        t = self.t
+        if not (x.is_cuda and x.dtype == th.float32):
+            return odeint_rk4(_fn, x, t)
+        n = len(t) - 1
+        dts = t[1:] - t[:-1]
+        third, eighth = dts * _ONE_THIRD, dts * 0.125
+        # per step (x, m0, m1, noise) weights of: y + dt/3 k1 | y + dt k2 - dt/3 k1 | y + dt k1 - dt k2 + dt k3 |
+        # acc = y + dt/8 k1 + 3dt/8 k2 + 3dt/8 k3 | acc + dt/8 k4
+        w = th.zeros(n, 5, 4)
+        w[:, :, 0] = 1.0
+        w[:, 0, 1] = third
+        w[:, 1, 1], w[:, 1, 2] = dts, -third
+        w[:, 2, 1], w[:, 2, 2], w[:, 2, 3] = dts, -dts, dts
+        w[:, 3, 1], w[:, 3, 2], w[:, 3, 3] = eighth, 3 * eighth, 3 * eighth
+        w[:, 4, 1] = eighth
+        tab = w[:, :, None, :].expand(n, 5, B, 4).contiguous().to(device)
+        upd = ops.sampler_affine_update
+        ys = [x]
+        for i in range(n):
+            t0, dt, c = t[i], dts[i], tab[i]
+            y = ys[-1].contiguous()
+            k1 = _fn(t0, y).float().contiguous()
+            k2 = _fn(t0 + dt * _ONE_THIRD, upd(y, c[0], k1)).float().contiguous()
+            k3 = _fn(t0 + dt * _TWO_THIRDS, upd(y, c[1], k2, k1)).float().contiguous()
+            k4 = _fn(t[i + 1], upd(y, c[2], k1, k2, k3)).float().contiguous()
+            ys.append(upd(upd(y, c[3], k1, k2, k3), c[4], k4))
+        return th.stack(ys, 0)
 
 
 class Sampler:
