@@ -506,15 +506,29 @@ def sample_flow_batched(model, c: dict, uc: dict, num_samples: int, seed: int = 
     return y[:P * N].reshape(P, N, *shape), stats
 
 
+def _condition_list(conditioner, cond_key, prompts, num_samples, dev):
+    """condition_prompt once per prompt, in order, stacked condition-major: (c, uc) with (P*N, ...) per tensor key."""
+    cs, ucs = zip(*(condition_prompt(conditioner, cond_key, p, num_samples, device=dev) for p in prompts))
+    c = {k: torch.cat([ci[k] for ci in cs]) if isinstance(cs[0][k], torch.Tensor) else cs[0][k] for k in cs[0]}
+    uc = {k: torch.cat([ui[k] for ui in ucs]) if isinstance(ucs[0][k], torch.Tensor) else ucs[0][k] for k in ucs[0]}
+    return c, uc
+
+
+def _own(x, dev, dtype):
+    """A condition's own copy on `dev` in `dtype` (a tensor, or a dict of them): the conditioner's kernels want
+    16-byte aligned rows, and aug_c rotates the cameras of this copy in place."""
+    if isinstance(x, dict):
+        return {k: _own(v, dev, dtype) for k, v in x.items()}
+    return x.to(dev).to(dtype).clone()
+
+
 @torch.no_grad()
 def _conds_to_3d(conditioner, model, decoder, cond_key, prompts, cameras, num_samples, seed, num_steps, cfg_scale,
                  resolution, dtype, sde, sampling_method):
     """`_cond_to_3d` for a list of conditions: the conditioner once per condition, in order, one batched sample,
     then decode and render of every latent.  The render noise is one device draw for the batch."""
     dev = next(model.parameters()).device
-    cs, ucs = zip(*(condition_prompt(conditioner, cond_key, p, num_samples, device=dev) for p in prompts))
-    c = {k: torch.cat([ci[k] for ci in cs]) if isinstance(cs[0][k], torch.Tensor) else cs[0][k] for k in cs[0]}
-    uc = {k: torch.cat([ui[k] for ui in ucs]) if isinstance(ucs[0][k], torch.Tensor) else ucs[0][k] for k in ucs[0]}
+    c, uc = _condition_list(conditioner, cond_key, prompts, num_samples, dev)
     latents, stats = sample_flow_batched(model, c, uc, num_samples, seed=seed, num_steps=num_steps,
                                          cfg_scale=cfg_scale, dtype=dtype, sde=sde, sampling_method=sampling_method)
     P, N = latents.shape[:2]
@@ -532,7 +546,7 @@ def images_to_3d(conditioner, model, decoder, images: torch.Tensor, cameras: tor
     sample_flow_batched.
     Returns (latents (P, N, 12, 32, 32), render dict with (P, N, 24, ...) tensors, per-image stats)."""
     dev = next(model.parameters()).device
-    imgs = [images[i:i + 1].to(dev).to(dtype).clone() for i in range(images.shape[0])]   # own, aligned buffers
+    imgs = [_own(images[i:i + 1], dev, dtype) for i in range(images.shape[0])]
     return _conds_to_3d(conditioner, model, decoder, "img", imgs, cameras, num_samples, seed, num_steps, cfg_scale,
                         resolution, dtype, sde, sampling_method)
 
@@ -548,10 +562,109 @@ def mvs_to_3d(conditioner, model, decoder, mv_images: torch.Tensor, mv_cameras: 
     caller's `mv_cameras` is left as it is.  `sde`, `sampling_method`: see sample_flow_batched.  Returns as
     `images_to_3d`."""
     dev = next(model.parameters()).device
-    own = lambda x, i: x[i:i + 1].to(dev).to(dtype).clone()
-    prompts = [{"img": own(mv_images, i), "c": own(mv_cameras, i)} for i in range(mv_images.shape[0])]
+    prompts = [_own({"img": mv_images[i:i + 1], "c": mv_cameras[i:i + 1]}, dev, dtype)
+               for i in range(mv_images.shape[0])]
     return _conds_to_3d(conditioner, model, decoder, "img-c", prompts, cameras, num_samples, seed, num_steps,
                         cfg_scale, resolution, dtype, sde, sampling_method)
+
+
+@torch.no_grad()
+def _conds_to_3d_sharded(conditioner, model, decoder, cond_key, P, host_prompt, cameras, *, num_samples, seed,
+                         num_steps, cfg_scale, resolution, dtype, sde, sampling_method, batch, with_depth, device,
+                         group, gather, sample_fn, render_fn, pack_fn):
+    """The body of images_to_3d_sharded / mvs_to_3d_sharded; host_prompt(i) is condition i as the caller holds it."""
+    dev = torch.device(device) if device is not None else next(model.parameters()).device
+    N = num_samples
+    lo, hi, per = shard_range(P, *_world_rank(group))
+    if sample_fn is None:
+        sample_fn = lambda c, uc: sample_flow_batched(model, c, uc, N, seed=seed, num_steps=num_steps,
+                                                      cfg_scale=cfg_scale, dtype=dtype, sde=sde,
+                                                      sampling_method=sampling_method)
+    if render_fn is None:
+        cams = cameras[:24].to(dev)
+        render_fn = lambda lat: decode_and_render(decoder, lat, cams, resolution)
+    if pack_fn is None:
+        pack_fn = _frame_packer(dev, with_depth)
+    frame_shape = (N, min(cameras.shape[0], 24), resolution, resolution * (2 if with_depth else 1), 3)
+    latents = torch.zeros(per, N, 12, 32, 32, device=dev)
+    stats: dict = {}
+
+    def run_batch(i0, i1):
+        c, uc = _condition_list(conditioner, cond_key, [_own(host_prompt(i), dev, dtype) for i in range(i0, i1)], N,
+                                dev)
+        lat, st = sample_fn(c, uc)
+        latents[i0 - lo:i1 - lo].copy_(lat)
+        for k, v in st.items():
+            if isinstance(v, list):                   # per-condition counts; batch_nfe belongs to one batch only
+                stats.setdefault(k, []).extend(v)
+        return pack_fn(render_fn(lat.reshape(-1, *lat.shape[2:]))).reshape(i1 - i0, *frame_shape)
+
+    # every rank draws the host RNG of all P conditions in order (aug_c), and applies only its own shard's draws
+    for i in range(lo):
+        conditioner.skip_unconditional_conditioning({cond_key: host_prompt(i)})
+    out = _sharded_frames(P, batch, frame_shape, dev, group, gather, run_batch)
+    for i in range(hi, P):
+        conditioner.skip_unconditional_conditioning({cond_key: host_prompt(i)})
+    return dict(latents=latents[:hi - lo], stats=stats, **out)
+
+
+@torch.no_grad()
+def images_to_3d_sharded(conditioner, model, decoder, images: torch.Tensor, cameras: torch.Tensor,
+                         num_samples: int = 4, seed: int = 42, num_steps: int = 250, cfg_scale: float = 4.0,
+                         resolution: int = 192, dtype=torch.float32, sde: dict | None = None,
+                         sampling_method: str = "dopri5", *, batch: int = 8, with_depth: bool = False, device=None,
+                         group=None, gather: bool = True, sample_fn=None, render_fn=None, pack_fn=None) -> dict:
+    """`images_to_3d` for P images (P, 3, H, W) sharded over the ranks of `group` (SURVEY 8d configuration 4).
+
+    Every rank holds all P images and owns the contiguous block [lo, hi) of shard_range(P, world, rank).  It works
+    through its block in local batches of at most `batch` images; a batch runs the conditioner once per image, in
+    order (only on this rank's images), sample_flow_batched (`sampling_method`, `sde` as in images_to_3d),
+    decode_and_render of `cameras[:24]` at `resolution`, and FrameSink.pack (image | colour-mapped depth side by side
+    with `with_depth`).  Each batch ends with ONE all_gather_into_tensor of its uint8 frames on a side stream, so the
+    gather overlaps the next batch; every rank makes the same number of trips, and ranks holding fewer images
+    contribute zero frames that are trimmed from the result.
+
+    Equal to one process: each image's initial noise is the draw sample_flow makes (flow_batch_noise), so nothing is
+    sliced across ranks, and its latents equal those of images_to_3d over the same image list up to the rounding of
+    the batched GEMMs (an adaptive solve is per image, so only the batch size can change them).  With world == 1
+    and batch >= P this is images_to_3d, bit for bit, renders included.  The renders of a run with several batches
+    use one device noise draw per batch, so they differ from images_to_3d's.
+
+    Returns {'latents': (n_local, N, 12, 32, 32), 'frames': uint8 (n_local, N, V, H, Wout, 3), 'frames_all': uint8
+    (P, N, V, H, Wout, 3) in image order on every rank (None with gather=False), 'shard': (lo, hi),
+    'gather_bytes_per_rank': int, 'stats': the per-image solver lists (nfe; accepted / rejected for an adaptive
+    method) of this rank's images}; V = min(24, len(cameras)), Wout = resolution (2 resolution with depth).
+    `sample_fn(c, uc) -> (latents, stats)`, `render_fn(latents (n*N, ...)) -> render dict` and `pack_fn(render dict)`
+    replace the three CUDA stages, and `device` the model's device (the gloo test drives this function's sharding,
+    condition order and gather with CPU stand-ins)."""
+    return _conds_to_3d_sharded(conditioner, model, decoder, "img", images.shape[0], lambda i: images[i:i + 1],
+                                cameras, num_samples=num_samples, seed=seed, num_steps=num_steps, cfg_scale=cfg_scale,
+                                resolution=resolution, dtype=dtype, sde=sde, sampling_method=sampling_method,
+                                batch=batch, with_depth=with_depth, device=device, group=group, gather=gather,
+                                sample_fn=sample_fn, render_fn=render_fn, pack_fn=pack_fn)
+
+
+@torch.no_grad()
+def mvs_to_3d_sharded(conditioner, model, decoder, mv_images: torch.Tensor, mv_cameras: torch.Tensor,
+                      cameras: torch.Tensor, num_samples: int = 4, seed: int = 42, num_steps: int = 250,
+                      cfg_scale: float = 4.0, resolution: int = 192, dtype=torch.float32, sde: dict | None = None,
+                      sampling_method: str = "dopri5", *, batch: int = 8, with_depth: bool = False, device=None,
+                      group=None, gather: bool = True, sample_fn=None, render_fn=None, pack_fn=None) -> dict:
+    """`mvs_to_3d` for P multi-view conditions, mv_images (P, V, 3, H, W) and mv_cameras (P, V, 25), sharded over the
+    ranks of `group` as images_to_3d_sharded shards images; arguments and results as there.
+
+    aug_c: the release conditioner (FrozenDinov2ImageEmbedderMVPlucker, aug_c=True) rotates cameras with draws from
+    Python `random` and `np.random`, per (condition, view) and in condition order.  So every rank makes the draws of
+    ALL P conditions in order -- conditioner.skip_unconditional_conditioning for each condition another rank owns --
+    and applies only those of its own conditions, on the device copy of their cameras, in `dtype`.  Each condition
+    therefore sees the rotations a single mvs_to_3d call gives it after the same seeds, and every rank leaves both
+    generators where that call leaves them.  The caller's `mv_cameras` is never rotated."""
+    return _conds_to_3d_sharded(conditioner, model, decoder, "img-c", mv_images.shape[0],
+                                lambda i: {"img": mv_images[i:i + 1], "c": mv_cameras[i:i + 1]}, cameras,
+                                num_samples=num_samples, seed=seed, num_steps=num_steps, cfg_scale=cfg_scale,
+                                resolution=resolution, dtype=dtype, sde=sde, sampling_method=sampling_method,
+                                batch=batch, with_depth=with_depth, device=device, group=group, gather=gather,
+                                sample_fn=sample_fn, render_fn=render_fn, pack_fn=pack_fn)
 
 
 @torch.no_grad()
@@ -654,14 +767,8 @@ def generate_sharded(model, decoder, c_all: dict, uc_all: dict, cameras: torch.T
     (P, V, H, Wout, 3) on every rank (None if not gathered), 'shard': (lo, hi), 'gather_bytes_per_rank': int}.
     `sample_fn / render_fn / pack_fn` replace the three CUDA stages (the world-size-2 gloo test drives the
     sharding, padding and gather logic of THIS function with CPU stand-ins)."""
-    import torch.distributed as dist
-    distributed = dist.is_available() and dist.is_initialized()
-    world = dist.get_world_size(group) if distributed else 1
-    rank = dist.get_rank(group) if distributed else 0
     P = c_all["crossattn"].shape[0]
-    lo, hi, per = shard_range(P, world, rank)
     dev = torch.device(device) if device is not None else next(model.parameters()).device
-    V = cameras.shape[0]
     g = torch.Generator().manual_seed(seed)
     randn_all = torch.randn(P, 12, 32, 32, generator=g)                      # identical on every rank
     if sample_fn is None:
@@ -669,14 +776,54 @@ def generate_sharded(model, decoder, c_all: dict, uc_all: dict, cameras: torch.T
     if render_fn is None:
         render_fn = lambda lat: decode_and_render(decoder, lat, cameras, resolution)
     if pack_fn is None:
-        from .frames import FrameSink
-        sink = FrameSink(dev)
-        pack_fn = lambda r: sink.pack(r["image_raw"], r["image_depth"] if with_depth else None)
-    Wout = resolution * (2 if with_depth else 1)
-    frames = torch.zeros(per, V, resolution, Wout, 3, dtype=torch.uint8, device=dev)
+        pack_fn = _frame_packer(dev, with_depth)
+    lo, hi, per = shard_range(P, *_world_rank(group))
     latents = torch.zeros(per, 12, 32, 32, device=dev)
+
+    def run_batch(i0, i1):
+        sl = slice(i0, i1)
+        x = randn_all[sl].to(dev, non_blocking=True)
+        c = {"crossattn": c_all["crossattn"][sl].to(dev, non_blocking=True)}
+        uc = {"crossattn": uc_all["crossattn"][sl].to(dev, non_blocking=True)}
+        lat = sample_fn(x, c, uc)
+        latents[i0 - lo:i1 - lo].copy_(lat)
+        return pack_fn(render_fn(lat))
+
+    out = _sharded_frames(P, batch, (cameras.shape[0], resolution, resolution * (2 if with_depth else 1), 3), dev,
+                          group, gather, run_batch)
+    return dict(latents=latents[:hi - lo], **out)
+
+
+def _world_rank(group) -> tuple[int, int]:
+    """(world size, rank) of `group`, or (1, 0) without an initialised process group."""
+    import torch.distributed as dist
+    if dist.is_available() and dist.is_initialized():
+        return dist.get_world_size(group), dist.get_rank(group)
+    return 1, 0
+
+
+def _frame_packer(dev, with_depth: bool):
+    """The default pack stage of the sharded pipelines: FrameSink.pack of image_raw (and image_depth)."""
+    from .frames import FrameSink
+    sink = FrameSink(dev)
+    return lambda r: sink.pack(r["image_raw"], r["image_depth"] if with_depth else None)
+
+
+def _sharded_frames(P: int, batch: int, frame_shape: tuple, dev, group, gather: bool, run_batch) -> dict:
+    """The batch loop and frame gather that every sharded pipeline shares.  This rank of `group` owns the contiguous
+    block [lo, hi) of shard_range(P, world, rank) and works through it in local batches of at most `batch` items:
+    run_batch(i0, i1) runs the global items [i0, i1) and returns their uint8 frames (i1 - i0, *frame_shape).  Every
+    rank makes ceil(per / batch) trips, including ranks that own fewer items or none; each trip ends with ONE
+    all_gather_into_tensor of the batch's frame rows (zeros past the rank's last item), issued on a side stream so
+    that it overlaps the next batch.  The padding rows are trimmed from the result.
+    Returns {'frames': (n_local, *frame_shape), 'frames_all': (P, *frame_shape) in item order on every rank (None if
+    not gathered), 'shard': (lo, hi), 'gather_bytes_per_rank': int}."""
+    import torch.distributed as dist
+    world, rank = _world_rank(group)
+    lo, hi, per = shard_range(P, world, rank)
+    frames = torch.zeros(per, *frame_shape, dtype=torch.uint8, device=dev)
     do_gather = gather and world > 1
-    frames_all = torch.empty(world, per, V, resolution, Wout, 3, dtype=torch.uint8, device=dev) if do_gather else None
+    frames_all = torch.empty(world, per, *frame_shape, dtype=torch.uint8, device=dev) if do_gather else None
     cuda = dev.type == "cuda"
     side = torch.cuda.Stream(device=dev) if (do_gather and cuda) else None
     pending = []
@@ -684,13 +831,7 @@ def generate_sharded(model, decoder, c_all: dict, uc_all: dict, cameras: torch.T
         b1 = min(b0 + batch, per)
         n_valid = max(0, min(hi - lo, b1) - b0)
         if n_valid > 0:
-            sl = slice(lo + b0, lo + b0 + n_valid)
-            x = randn_all[sl].to(dev, non_blocking=True)
-            c = {"crossattn": c_all["crossattn"][sl].to(dev, non_blocking=True)}
-            uc = {"crossattn": uc_all["crossattn"][sl].to(dev, non_blocking=True)}
-            lat = sample_fn(x, c, uc)
-            latents[b0:b0 + n_valid].copy_(lat)
-            frames[b0:b0 + n_valid].copy_(pack_fn(render_fn(lat)))
+            frames[b0:b0 + n_valid].copy_(run_batch(lo + b0, lo + b0 + n_valid))
         if do_gather:
             if b0 == 0 and b1 == per:                                        # one batch: gather straight into place
                 src, dst = frames, frames_all
@@ -712,6 +853,6 @@ def generate_sharded(model, decoder, c_all: dict, uc_all: dict, cameras: torch.T
     if side is not None:
         torch.cuda.current_stream(dev).wait_stream(side)
     n_local = hi - lo
-    out_all = frames_all.view(world * per, V, resolution, Wout, 3)[:P] if do_gather else (frames[:P] if gather else None)
-    return dict(latents=latents[:n_local], frames=frames[:n_local], frames_all=out_all, shard=(lo, hi),
+    out_all = frames_all.view(world * per, *frame_shape)[:P] if do_gather else (frames[:P] if gather else None)
+    return dict(frames=frames[:n_local], frames_all=out_all, shard=(lo, hi),
                 gather_bytes_per_rank=int(frames.numel()) if do_gather else 0)

@@ -155,6 +155,17 @@ class GeneralConditioner(nn.Module):
             embedder.ucg_rate = rate
         return c, uc
 
+    def skip_unconditional_conditioning(self, batch_c: Dict, batch_uc: Optional[Dict] = None) -> None:
+        """Advances the global host generators (`random`, `np.random`) as get_unconditional_conditioning(batch_c,
+        batch_uc) does, without running any embedder: every embedder with a `draw_augmentation` makes the draws of its
+        conditional pass, then those of its unconditional pass.  A sharded run calls it for each condition another
+        rank conditions, so that its own conditions get the draws a single process gives them."""
+        for batch in (batch_c, batch_c if batch_uc is None else batch_uc):
+            for embedder in self.embedders:
+                draw = getattr(embedder, "draw_augmentation", None)
+                if draw is not None and getattr(embedder, "input_key", None) is not None:
+                    draw(batch[embedder.input_key])
+
 
 # --------------------------------------------------------------------------------------------- helpers
 def _strip(sd: dict, *prefixes: str) -> dict:
@@ -682,13 +693,18 @@ class FrozenDinov2ImageEmbedderMVPlucker(FrozenDinov2ImageEmbedder):
         return super().preprocess(x)
 
     @staticmethod
-    def random_rotate_c(c: torch.Tensor) -> torch.Tensor:
-        """reference :1049-1076: a random rotation about z or y (InstantMesh's camera augmentation) applied to the
-        cam2world of one (25,) camera row, in the row's dtype.  RNG: np.random.uniform, then random.random()."""
-        intrinsics, c2ws = c[16:], c[:16].reshape(4, 4)
+    def draw_rotation() -> tuple:
+        """The draws of random_rotate_c: (angle, about_z) from np.random.uniform(0, 2 pi), then random.random() > 0.5."""
         degree = np.random.uniform(0, math.pi * 2)
+        return degree, random.random() > 0.5
+
+    @staticmethod
+    def rotate_c(c: torch.Tensor, degree, about_z: bool) -> torch.Tensor:
+        """The rotation of random_rotate_c for given draws: about z or y by `degree`, applied to the cam2world of one
+        (25,) camera row on its device, in its dtype."""
+        intrinsics, c2ws = c[16:], c[:16].reshape(4, 4)
         cs, sn = np.cos(degree), np.sin(degree)
-        if random.random() > 0.5:
+        if about_z:
             rot = [[cs, -sn, 0, 0], [sn, cs, 0, 0], [0, 0, 1, 0], [0, 0, 0, 1]]
         else:
             rot = [[cs, 0, sn, 0], [0, 1, 0, 0], [-sn, 0, cs, 0], [0, 0, 0, 1]]
@@ -696,13 +712,36 @@ class FrozenDinov2ImageEmbedderMVPlucker(FrozenDinov2ImageEmbedder):
         return torch.cat([torch.matmul(rot, c2ws).reshape(-1), intrinsics])
 
     @classmethod
+    def random_rotate_c(cls, c: torch.Tensor) -> torch.Tensor:
+        """reference :1049-1076: a random rotation about z or y (InstantMesh's camera augmentation) applied to the
+        cam2world of one (25,) camera row, in the row's dtype.  RNG: np.random.uniform, then random.random()."""
+        return cls.rotate_c(c, *cls.draw_rotation())
+
+    @classmethod
+    def draw_camera_augmentation(cls, B: int, V: int) -> list:
+        """The host RNG draws of augment_cameras on a (B, V, 25) batch, in its order: per (b, v) random.random() > 0.6
+        decides, and a hit draws the rotation (draw_rotation).  Returns B lists of V entries, (degree, about_z) or
+        None.  Nothing is applied, so a caller can advance `random` and `np.random` exactly as augment_cameras would."""
+        return [[cls.draw_rotation() if random.random() > 0.6 else None for _ in range(V)] for _ in range(B)]
+
+    @classmethod
+    def apply_camera_augmentation(cls, c: torch.Tensor, draws: list) -> torch.Tensor:
+        """Rotates the cameras of c (B, V, 25) in place by draws of draw_camera_augmentation(B, V), on c's device, in
+        its dtype.  Draws no random numbers."""
+        for b, row in enumerate(draws):
+            for v, d in enumerate(row):
+                if d is not None:
+                    c[b, v] = cls.rotate_c(c[b, v], *d)
+        return c
+
+    @classmethod
     def augment_cameras(cls, c: torch.Tensor) -> torch.Tensor:
         """aug_c (reference :1084-1088): every camera of c (B, V, 25) is rotated, in place, with probability 0.4."""
-        for b in range(c.shape[0]):
-            for v in range(c.shape[1]):
-                if random.random() > 0.6:
-                    c[b, v] = cls.random_rotate_c(c[b, v])
-        return c
+        return cls.apply_camera_augmentation(c, cls.draw_camera_augmentation(c.shape[0], c.shape[1]))
+
+    def draw_augmentation(self, img_c) -> list | None:
+        """The host RNG draws forward(img_c) makes (its aug_c camera draws, or none), made without running it."""
+        return self.draw_camera_augmentation(*img_c["c"].shape[:2]) if self.aug_c else None
 
     def encode_with_vision_transformer(self, img, cams=None, **kwargs):
         """(B*V, 3, H, W) views + (B*V, 25) cameras -> patch tokens (B*V, 256, width)."""
